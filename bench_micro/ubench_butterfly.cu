@@ -13,29 +13,26 @@ template <int MODE>
 __global__ void __launch_bounds__(256) kb(u64* out, u64 q, u64 nq, u64 qb, u64 seed, int rounds) {
   u64 a[16];
   Hb1TwReg tw;
-#pragma unroll
-  for (int i = 0; i < 16; i++) a[i] = (seed + threadIdx.x * 977 + i * 131 + blockIdx.x) % q;
-#pragma unroll
-  for (int i = 0; i < 15; i++) { u64 w = (seed * (i + 3) + 12345) % q; tw.t[i] = make_ulonglong2(w, (u64)(((unsigned __int128)w << 64) / q)); }
+  hb1_unroll<16>([&](auto i) { a[i] = (seed + threadIdx.x * 977 + i * 131 + blockIdx.x) % q; });
+  tw.load([&](int k, int g) {
+    const int i = (1 << k) - 1 + g;
+    u64 w = (seed * (i + 3) + 12345) % q;
+    return make_ulonglong2(w, (u64)(((unsigned __int128)w << 64) / q));
+  });
   for (int r = 0; r < rounds; r++) {
     Hb1Mod M; M.nq = nq; M.qb = qb; M.qb2 = qb + qb; M.qt = (unsigned)((q - 1) >> 52); M.qsh = 20;   // q = 237*2^52 + 1
     if (MODE == 0) hb1_r16_fwd<false>(a, tw, M);
     else if (MODE == 1) hb1_r16_inv<false>(a, tw, M);
     else if (MODE == 3) hb1_r16_fwd<true>(a, tw, M);
     else {
-#pragma unroll
-      for (int k = 0; k < 4; k++) { const int d = 8 >> k;
-#pragma unroll
-        for (int g = 0; g < (1 << k); g++) { const ulonglong2 w = tw.get(k, g);
-#pragma unroll
-          for (int o = 0; o < d; o++) ct_exact(a[g * 2 * d + o], a[g * 2 * d + o + d], w.x, w.y, q, q + q); } }
+      hb1_unroll<4>([&](auto k) { constexpr int d = 8 >> k;
+        hb1_unroll<(1 << k)>([&](auto g) { const ulonglong2 w = tw.template get<k, g>();
+          hb1_unroll<d>([&](auto o) { ct_exact(a[g * 2 * d + o], a[g * 2 * d + o + d], w.x, w.y, q, q + q); }); }); });
     }
-#pragma unroll
-    for (int i = 0; i < 16; i++) a[i] = hb1_csub_hi(hb1_csub_hi(a[i], qb), qb);   // keep bounded between rounds
+    hb1_unroll<16>([&](auto i) { a[i] = hb1_csub_hi(hb1_csub_hi(a[i], qb), qb); });   // keep bounded between rounds
   }
   u64 s = 0;
-#pragma unroll
-  for (int i = 0; i < 16; i++) s ^= a[i];
+  hb1_unroll<16>([&](auto i) { s ^= a[i]; });
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 // 128-bit MAC throughput

@@ -13,6 +13,7 @@
 //   k1_conv                 : fused iNTT-cols -> exact CRT -> NTT-cols with 64-thread groups
 //                             working on different rows concurrently.  needs n1 = 8
 #pragma once
+#include <utility>
 #include "hb_device.cuh"
 
 #define HB1_RS 17     // row stride inside a 256-element transform tile
@@ -136,41 +137,55 @@ __device__ __forceinline__ u64 hb1_canon_inv(u64 x, u64 q) {  // inverse network
   return hb1_csub(x, q);
 }
 
+// ---- compile-time unrolling ----------------------------------------------------------------
+// hb1_unroll<N>(f) calls f(HbC<0>{}), ..., f(HbC<N-1>{}): the index is a constant of the C++ program itself, so every
+// access to a per-thread array (the 16 residues, the twiddle pairs, the MAC accumulators) has a constant subscript and
+// the array lives in registers.  #pragma unroll only asks the loop unroller, whose decisions depend on the target: on
+// sm_90a it left the nested network loops partly rolled and put a[16] and the twiddles in local memory (a 368-byte stack
+// frame in every transform kernel), which the sm_100a code generation did not.  Every 16-wide loop around the
+// network uses this instead of #pragma unroll.
+template <int I> struct HbC {
+  static constexpr int value = I;
+  __device__ constexpr operator int() const { return I; }
+};
+template <class F, int... I>
+__device__ __forceinline__ void hb1_unroll_seq(F&& f, std::integer_sequence<int, I...>) { (f(HbC<I>{}), ...); }
+template <int N, class F>
+__device__ __forceinline__ void hb1_unroll(F&& f) { hb1_unroll_seq(f, std::make_integer_sequence<int, N>{}); }
+
 // 4 forward stages on 16 registers; twiddle of stage k (distance 8>>k), group g is tw[(1<<k)-1+g]
 struct Hb1TwReg {
   ulonglong2 t[15];
-  __device__ __forceinline__ ulonglong2 get(int k, int g) const { return t[(1 << k) - 1 + g]; }
+  template <int K, int G> __device__ __forceinline__ ulonglong2 get() const { return t[(1 << K) - 1 + G]; }
+  // t[(1<<k)-1+g] = f(k, g) for every stage k and group g
+  template <class F> __device__ __forceinline__ void load(F&& f) {
+    hb1_unroll<4>([&](auto k) { hb1_unroll<(1 << k)>([&](auto g) { t[(1 << k) - 1 + g] = f((int)k, (int)g); }); });
+  }
 };
 // twiddles read through a pointer per stage (uniform/broadcast loads or shared memory)
 struct Hb1TwPtr {
   const ulonglong2* p[4];
-  __device__ __forceinline__ ulonglong2 get(int k, int g) const { return p[k][g]; }
+  template <int K, int G> __device__ __forceinline__ ulonglong2 get() const { return p[K][G]; }
 };
 template <bool SP, class TW>
 __device__ __forceinline__ void hb1_r16_fwd(u64 (&a)[16], const TW& tw, const Hb1Mod& M) {
-#pragma unroll
-  for (int k = 0; k < 4; k++) {
-    const int d = 8 >> k;
-#pragma unroll
-    for (int g = 0; g < (1 << k); g++) {
-      const ulonglong2 w = tw.get(k, g);
-#pragma unroll
-      for (int o = 0; o < d; o++) hb1_ct<SP>(a[g * 2 * d + o], a[g * 2 * d + o + d], w.x, w.y, M);
-    }
-  }
+  hb1_unroll<4>([&](auto k) {
+    constexpr int d = 8 >> k;
+    hb1_unroll<(1 << k)>([&](auto g) {
+      const ulonglong2 w = tw.template get<k, g>();
+      hb1_unroll<d>([&](auto o) { hb1_ct<SP>(a[g * 2 * d + o], a[g * 2 * d + o + d], w.x, w.y, M); });
+    });
+  });
 }
 template <bool SP, class TW>
 __device__ __forceinline__ void hb1_r16_inv(u64 (&a)[16], const TW& tw, const Hb1Mod& M) {
-#pragma unroll
-  for (int k = 3; k >= 0; k--) {
-    const int d = 8 >> k;
-#pragma unroll
-    for (int g = 0; g < (1 << k); g++) {
-      const ulonglong2 w = tw.get(k, g);
-#pragma unroll
-      for (int o = 0; o < d; o++) hb1_gs<SP>(a[g * 2 * d + o], a[g * 2 * d + o + d], w.x, w.y, M);
-    }
-  }
+  hb1_unroll<4>([&](auto kr) {
+    constexpr int k = 3 - kr, d = 8 >> k;
+    hb1_unroll<(1 << k)>([&](auto g) {
+      const ulonglong2 w = tw.template get<k, g>();
+      hb1_unroll<d>([&](auto o) { hb1_gs<SP>(a[g * 2 * d + o], a[g * 2 * d + o + d], w.x, w.y, M); });
+    });
+  });
 }
 __device__ __forceinline__ unsigned hb1_brev4(unsigned x) {
   return ((x & 1u) << 3) | ((x & 2u) << 1) | ((x & 4u) >> 1) | ((x & 8u) >> 3);
@@ -264,8 +279,7 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restric
   Hb1Unit cur = hb1_unit(ubeg, G, J.nitems);
   {
     const u64* src = src_ptr(cur);
-#pragma unroll
-    for (int r = 0; r < 16; r++) hb1_cp8(S + own + HB1_RS * r, src + 16 * r);
+    hb1_unroll<16>([&](auto r) { hb1_cp8(S + own + HB1_RS * r, src + 16 * r); });
   }
   hb1_cp_commit();
   int key = -1, buf = 0;
@@ -284,11 +298,7 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restric
         int g = e - ((1 << k) - 1);
         TW1[blk1 * 16 + e] = P.fw[((size_t)1 << (n1 + k)) + ((size_t)b1 << k) + g];
       }
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-#pragma unroll
-        for (int g = 0; g < (1 << k); g++)
-          tw2.t[(1 << k) - 1 + g] = P.fw[((size_t)1 << (n1 + 4 + k)) + ((size_t)b2 << (4 + k)) + ((size_t)hi << k) + g];
+      tw2.load([&](int k, int g) { return P.fw[((size_t)1 << (n1 + 4 + k)) + ((size_t)b2 << (4 + k)) + ((size_t)hi << k) + g]; });
       __syncthreads();  // TW1 visible (the previous unit's trailing barrier ordered its last use)
     }
     u64* Sb = S + buf * HB1_STAGE;
@@ -297,8 +307,7 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restric
     const bool epi = epi1 || (epi3 && sc != 0);           // uniform per unit
     u64* old = epi3 ? J.dst2[cur.it] + doff : dst;        // where the value to be updated lives
     if (epi) {
-#pragma unroll
-      for (int l = 0; l < 16; l++) hb1_cp8(O + l * 256 + tid, old + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1));
+      hb1_unroll<16>([&](auto l) { hb1_cp8(O + l * 256 + tid, old + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1)); });
     }
     hb1_cp_commit();
     Hb1Unit nxt = cur;
@@ -306,24 +315,19 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restric
       nxt = hb1_unit_next(cur, G, J.nitems);
       const u64* src = src_ptr(nxt);
       u64* Sn = S + (buf ^ 1) * HB1_STAGE;
-#pragma unroll
-      for (int r = 0; r < 16; r++) hb1_cp8(Sn + own + HB1_RS * r, src + 16 * r);
+      hb1_unroll<16>([&](auto r) { hb1_cp8(Sn + own + HB1_RS * r, src + 16 * r); });
     }
     hb1_cp_commit();
     hb1_cp_wait<2>();   // this unit's inputs have landed (issued one iteration ago)
     u64 a[16];
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = Sb[own + HB1_RS * r];
+    hb1_unroll<16>([&](auto r) { a[r] = Sb[own + HB1_RS * r]; });
     hb1_r16_fwd<SP>(a, tw1, M);
-#pragma unroll
-    for (int r = 0; r < 16; r++) Sb[own + HB1_RS * r] = a[r];
+    hb1_unroll<16>([&](auto r) { Sb[own + HB1_RS * r] = a[r]; });
     __syncthreads();
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = Sb[blk2 * HB1_BS + HB1_RS * hi + l];
+    hb1_unroll<16>([&](auto l) { a[l] = Sb[blk2 * HB1_BS + HB1_RS * hi + l]; });
     hb1_r16_fwd<SP>(a, tw2, M);
     hb1_cp_wait<1>();   // old destination values (epilogue) have landed
-#pragma unroll
-    for (int l = 0; l < 16; l++) {
+    hb1_unroll<16>([&](auto l) {
       const size_t o = (size_t)((hb1_brev4(l) << 4) | hrev) << n1;   // brev8(16*hi + l) * N1
       if (epi) {
         u64 v = hb1_shoup4<SP>(O[l * 256 + tid] - a[l] + (M.qb2 + M.qb), sc, sc_s, M);   // (old - x) * P^-1, x in [0, 8q + 2^32), old < 4q
@@ -331,7 +335,7 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restric
         old[o] = v;
       }
       if (!epi1) dst[o] = lazy ? a[l] : hb1_canon_fwd(a[l], q, M.qb);
-    }
+    });
     __syncthreads();   // exchange reads of Sb / TW1 done before they are overwritten
     cur = nxt;
   }
@@ -363,8 +367,7 @@ __global__ void __launch_bounds__(256, 2) k1_inv_blk(const HbPrimeDev* __restric
   Hb1Unit cur = hb1_unit(ubeg, G, J.nitems);
   {
     const u64* src = src_ptr(cur);
-#pragma unroll
-    for (int l = 0; l < 16; l++) hb1_cp8(S + own + l, src + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1));
+    hb1_unroll<16>([&](auto l) { hb1_cp8(S + own + l, src + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1)); });
   }
   hb1_cp_commit();
   int key = -1, buf = 0;
@@ -384,11 +387,7 @@ __global__ void __launch_bounds__(256, 2) k1_inv_blk(const HbPrimeDev* __restric
         int g = e - ((1 << k) - 1);
         TW1[blk1 * 16 + e] = P.iw[((size_t)1 << (n1 + k)) + ((size_t)b1 << k) + g];
       }
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-#pragma unroll
-        for (int g = 0; g < (1 << k); g++)
-          tw2.t[(1 << k) - 1 + g] = P.iw[((size_t)1 << (n1 + 4 + k)) + ((size_t)b2 << (4 + k)) + ((size_t)hi << k) + g];
+      tw2.load([&](int k, int g) { return P.iw[((size_t)1 << (n1 + 4 + k)) + ((size_t)b2 << (4 + k)) + ((size_t)hi << k) + g]; });
       __syncthreads();
     }
     u64* Sb = S + buf * HB1_STAGE;
@@ -397,24 +396,19 @@ __global__ void __launch_bounds__(256, 2) k1_inv_blk(const HbPrimeDev* __restric
       nxt = hb1_unit_next(cur, G, J.nitems);
       const u64* src = src_ptr(nxt);
       u64* Sn = S + (buf ^ 1) * HB1_STAGE;
-#pragma unroll
-      for (int l = 0; l < 16; l++) hb1_cp8(Sn + own + l, src + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1));
+      hb1_unroll<16>([&](auto l) { hb1_cp8(Sn + own + l, src + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1)); });
     }
     hb1_cp_commit();
     hb1_cp_wait<1>();
     u64 a[16];
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = Sb[own + l];
+    hb1_unroll<16>([&](auto l) { a[l] = Sb[own + l]; });
     hb1_r16_inv<SP>(a, tw2, M);
-#pragma unroll
-    for (int l = 0; l < 16; l++) Sb[own + l] = a[l];
+    hb1_unroll<16>([&](auto l) { Sb[own + l] = a[l]; });
     __syncthreads();
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = Sb[blk1 * HB1_BS + HB1_RS * r + lo];
+    hb1_unroll<16>([&](auto r) { a[r] = Sb[blk1 * HB1_BS + HB1_RS * r + lo]; });
     hb1_r16_inv<SP>(a, tw1, M);
     u64* dst = J.dst[cur.it] + ((size_t)J.rows.prime[cur.rowi] << J.logN) + ((size_t)b1 << 8) + lo;
-#pragma unroll
-    for (int r = 0; r < 16; r++) dst[16 * r] = J.epi == 2 ? a[r] : hb1_canon_inv(a[r], q);   // epi 2: the consumer is a register kernel (lazy values are fine)
+    hb1_unroll<16>([&](auto r) { dst[16 * r] = J.epi == 2 ? a[r] : hb1_canon_inv(a[r], q); });   // epi 2: the consumer is a register kernel (lazy values are fine)
     __syncthreads();
     cur = nxt;
   }
@@ -450,25 +444,18 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_cols(const HbPrimeDev* __restri
   Hb1TwPtr tw1;
   tw1.p[0] = P.fw + 1; tw1.p[1] = P.fw + 2; tw1.p[2] = P.fw + 4; tw1.p[3] = P.fw + 8;
   Hb1TwReg tw2;
-#pragma unroll
-  for (int k = 0; k < 4; k++)
-#pragma unroll
-    for (int g = 0; g < (1 << k); g++) tw2.t[(1 << k) - 1 + g] = P.fw[(16 << k) + (x << k) + g];
+  tw2.load([&](int k, int g) { return P.fw[(16 << k) + (x << k) + g]; });
   for (int it = blockIdx.z; it < J.nitems; it += gridDim.z) {
     const u64* src = J.src[it] + rowoff + c0 + c;
     u64* dst = J.dst[it] + rowoff + c0 + c;
     u64 a[16];
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = src[(size_t)(16 * r + x) << 8];
+    hb1_unroll<16>([&](auto r) { a[r] = src[(size_t)(16 * r + x) << 8]; });
     hb1_r16_fwd<SP>(a, tw1, M);
-#pragma unroll
-    for (int r = 0; r < 16; r++) T[c * HB1_BS + HB1_RS * r + x] = a[r];
+    hb1_unroll<16>([&](auto r) { T[c * HB1_BS + HB1_RS * r + x] = a[r]; });
     __syncthreads();
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = T[c * HB1_BS + HB1_RS * x + l];
+    hb1_unroll<16>([&](auto l) { a[l] = T[c * HB1_BS + HB1_RS * x + l]; });
     hb1_r16_fwd<SP>(a, tw2, M);
-#pragma unroll
-    for (int l = 0; l < 16; l++) dst[(size_t)(16 * x + l) << 8] = a[l];   // lazy, [0, 8q + 2^32): the consumer is always k1_fwd_blk
+    hb1_unroll<16>([&](auto l) { dst[(size_t)(16 * x + l) << 8] = a[l]; });   // lazy, [0, 8q + 2^32): the consumer is always k1_fwd_blk
     __syncthreads();
   }
 }
@@ -486,31 +473,24 @@ __global__ void __launch_bounds__(256, 2) k1_inv_cols(const HbPrimeDev* __restri
   Hb1TwPtr tw1;
   tw1.p[0] = P.iw + 1; tw1.p[1] = P.iw + 2; tw1.p[2] = P.iw + 4; tw1.p[3] = P.iw + 8;
   Hb1TwReg tw2;
-#pragma unroll
-  for (int k = 0; k < 4; k++)
-#pragma unroll
-    for (int g = 0; g < (1 << k); g++) tw2.t[(1 << k) - 1 + g] = P.iw[(16 << k) + (x << k) + g];
+  tw2.load([&](int k, int g) { return P.iw[(16 << k) + (x << k) + g]; });
   for (int it = blockIdx.z; it < J.nitems; it += gridDim.z) {
     const u64* src = J.src[it] + rowoff + c0 + c;
     u64* dst = J.dst[it] + rowoff + c0 + c;
     u64 a[16];
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = src[(size_t)(16 * x + l) << 8];
+    hb1_unroll<16>([&](auto l) { a[l] = src[(size_t)(16 * x + l) << 8]; });
     hb1_r16_inv<SP>(a, tw2, M);
-#pragma unroll
-    for (int l = 0; l < 16; l++) T[c * HB1_BS + HB1_RS * x + l] = a[l];
+    hb1_unroll<16>([&](auto l) { T[c * HB1_BS + HB1_RS * x + l] = a[l]; });
     __syncthreads();
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = T[c * HB1_BS + HB1_RS * r + x];
+    hb1_unroll<16>([&](auto r) { a[r] = T[c * HB1_BS + HB1_RS * r + x]; });
     hb1_r16_inv<SP>(a, tw1, M);
     const u64 fm = J.has_scal ? J.scal[blockIdx.y] : P.ninv, fs = J.has_scal ? J.scal_s[blockIdx.y] : P.ninv_s;
-#pragma unroll
-    for (int r = 0; r < 16; r++) {
+    hb1_unroll<16>([&](auto r) {
       const u64 v = hb_mul_shoup(a[r], fm, fs, q);
       const size_t o = (size_t)(16 * r + x) << 8;
       dst[o] = v;
       for (int p = 0; p < J.npeers; p++) J.peer[p][it][rowoff + c0 + c + o] = v;
-    }
+    });
     __syncthreads();
   }
 }
@@ -556,11 +536,9 @@ __global__ void __launch_bounds__(640, 1) k1_conv(const HbPrimeDev* __restrict__
     const u64* s = src + ((size_t)pi << J.logN) + c0 + c;
     u64* Yj = Y + (size_t)j * HB1_TS + c * HB1C_BS;
     u64 a[16];
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = s[(size_t)(16 * x + l) << 8];
+    hb1_unroll<16>([&](auto l) { a[l] = s[(size_t)(16 * x + l) << 8]; });
     if (J.src_is_y) {   // uniform per launch: no transform, just stage the tile
-#pragma unroll
-      for (int l = 0; l < 16; l++) Yj[HB1_RS * x + l] = a[l];
+      hb1_unroll<16>([&](auto l) { Yj[HB1_RS * x + l] = a[l]; });
       continue;
     }
     {
@@ -568,19 +546,16 @@ __global__ void __launch_bounds__(640, 1) k1_conv(const HbPrimeDev* __restrict__
       tw.p[0] = P.iw + 16 + x; tw.p[1] = P.iw + 32 + 2 * x; tw.p[2] = P.iw + 64 + 4 * x; tw.p[3] = P.iw + 128 + 8 * x;
       hb1_r16_inv<SP>(a, tw, M);
     }
-#pragma unroll
-    for (int l = 0; l < 16; l++) Yj[HB1_RS * x + l] = a[l];
+    hb1_unroll<16>([&](auto l) { Yj[HB1_RS * x + l] = a[l]; });
     hb_group_sync(grp, 64);
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = Yj[HB1_RS * r + x];
+    hb1_unroll<16>([&](auto r) { a[r] = Yj[HB1_RS * r + x]; });
     {
       Hb1TwPtr tw;
       tw.p[0] = P.iw + 1; tw.p[1] = P.iw + 2; tw.p[2] = P.iw + 4; tw.p[3] = P.iw + 8;
       hb1_r16_inv<SP>(a, tw, M);
     }
     const u64 t = cv->tn[j], ts = cv->tn_s[j];
-#pragma unroll
-    for (int r = 0; r < 16; r++) Yj[HB1_RS * r + x] = hb_mul_shoup(a[r], t, ts, q);
+    hb1_unroll<16>([&](auto r) { Yj[HB1_RS * r + x] = hb_mul_shoup(a[r], t, ts, q); });
   }
   __syncthreads();
   // ---- v (multiple of Q to subtract, incl. the BGV correction) per coefficient
@@ -602,11 +577,9 @@ __global__ void __launch_bounds__(640, 1) k1_conv(const HbPrimeDev* __restrict__
     u64 a[16];
     {
       const u64 negq = cv->negQ[t], posq = cv->Qmod[t];
-#pragma unroll
-      for (int h = 0; h < 2; h++) {   // two halves of 8 coefficients: 32 accumulator registers live
+      hb1_unroll<2>([&](auto h) {   // two halves of 8 coefficients: 32 accumulator registers live
         u64 ahi[8], alo[8];
-#pragma unroll
-        for (int r = 0; r < 8; r++) {
+        hb1_unroll<8>([&](auto r) {
           const i64 v = Vb[c * HB1_VS + 16 * (8 * h + r) + x];
           const u64 m = v >= 0 ? (u64)v : (u64)(-v);
           const u64 f = v >= 0 ? negq : posq;
@@ -615,16 +588,14 @@ __global__ void __launch_bounds__(640, 1) k1_conv(const HbPrimeDev* __restrict__
             const u64 p1 = hb1_mulwide((unsigned)m, (unsigned)(f >> 32)) + (p0 >> 32);
             alo[r] = (p1 << 32) | (unsigned)p0; ahi[r] = p1 >> 32;
           } else { alo[r] = m * f; ahi[r] = __umul64hi(m, f); }
-        }
+        });
         for (int j = 0; j < n; j++) {
           const u64 cj = ct[j];
           const u64* Yj = Y + (size_t)j * HB1_TS + c * HB1C_BS + x + HB1_RS * 8 * h;
-#pragma unroll
-          for (int r = 0; r < 8; r++) hb1_mac128(ahi[r], alo[r], Yj[HB1_RS * r], cj);
+          hb1_unroll<8>([&](auto r) { hb1_mac128(ahi[r], alo[r], Yj[HB1_RS * r], cj); });
         }
-#pragma unroll
-        for (int r = 0; r < 8; r++) a[8 * h + r] = hb_reduce128_lazy(ahi[r], alo[r], P);   // [0,4q): fine for the CT network
-      }
+        hb1_unroll<8>([&](auto r) { a[8 * h + r] = hb_reduce128_lazy(ahi[r], alo[r], P); });   // [0,4q): fine for the CT network
+      });
     }
     {
       Hb1TwPtr tw;
@@ -632,19 +603,16 @@ __global__ void __launch_bounds__(640, 1) k1_conv(const HbPrimeDev* __restrict__
       hb1_r16_fwd<SP>(a, tw, M);
     }
     hb_group_sync(grp, 64);   // previous target's pass-2 reads of Wg are complete
-#pragma unroll
-    for (int r = 0; r < 16; r++) Wg[HB1_RS * r + x] = a[r];
+    hb1_unroll<16>([&](auto r) { Wg[HB1_RS * r + x] = a[r]; });
     hb_group_sync(grp, 64);
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = Wg[HB1_RS * x + l];
+    hb1_unroll<16>([&](auto l) { a[l] = Wg[HB1_RS * x + l]; });
     {
       Hb1TwPtr tw;
       tw.p[0] = P.fw + 16 + x; tw.p[1] = P.fw + 32 + 2 * x; tw.p[2] = P.fw + 64 + 4 * x; tw.p[3] = P.fw + 128 + 8 * x;
       hb1_r16_fwd<SP>(a, tw, M);
     }
     u64* d = dst + ((size_t)pi << J.logN) + c0 + c;
-#pragma unroll
-    for (int l = 0; l < 16; l++) d[(size_t)(16 * x + l) << 8] = a[l];   // lazy: k1_fwd_blk finishes the transform
+    hb1_unroll<16>([&](auto l) { d[(size_t)(16 * x + l) << 8] = a[l]; });   // lazy: k1_fwd_blk finishes the transform
   }
 }
 
@@ -683,25 +651,21 @@ __global__ void __launch_bounds__(640, 1) k1_conv1(const HbPrimeDev* __restrict_
     const u64* s = src + ((size_t)J.src_prime << J.logN) + c0 + 4 * qd + c;
     u64* Yq = Y + (size_t)qd * HB1_TS + c * HB1C_BS;
     u64 a[16];
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = s[(size_t)(16 * x + l) << 8];
+    hb1_unroll<16>([&](auto l) { a[l] = s[(size_t)(16 * x + l) << 8]; });
     {
       Hb1TwPtr tw;
       tw.p[0] = PS.iw + 16 + x; tw.p[1] = PS.iw + 32 + 2 * x; tw.p[2] = PS.iw + 64 + 4 * x; tw.p[3] = PS.iw + 128 + 8 * x;
       hb1_r16_inv<SP>(a, tw, M);
     }
-#pragma unroll
-    for (int l = 0; l < 16; l++) Yq[HB1_RS * x + l] = a[l];
+    hb1_unroll<16>([&](auto l) { Yq[HB1_RS * x + l] = a[l]; });
     hb_group_sync(grp, 64);
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = Yq[HB1_RS * r + x];
+    hb1_unroll<16>([&](auto r) { a[r] = Yq[HB1_RS * r + x]; });
     {
       Hb1TwPtr tw;
       tw.p[0] = PS.iw + 1; tw.p[1] = PS.iw + 2; tw.p[2] = PS.iw + 4; tw.p[3] = PS.iw + 8;
       hb1_r16_inv<SP>(a, tw, M);
     }
-#pragma unroll
-    for (int r = 0; r < 16; r++) Yq[HB1_RS * r + x] = hb_mul_shoup(a[r], J.ninv, J.ninv_s, PS.q);
+    hb1_unroll<16>([&](auto r) { Yq[HB1_RS * r + x] = hb_mul_shoup(a[r], J.ninv, J.ninv_s, PS.q); });
   }
   __syncthreads();
   // ---- targets
@@ -716,32 +680,28 @@ __global__ void __launch_bounds__(640, 1) k1_conv1(const HbPrimeDev* __restrict_
     const u64* Yq = Y + (size_t)qd * HB1_TS + c * HB1C_BS + x;
     const bool nored = J.nored[t] != 0;         // uniform per target: same-size primes (every ctxt / special prime of a chain)
     u64 a[16];
-#pragma unroll
-    for (int r = 0; r < 16; r++) {
+    hb1_unroll<16>([&](auto r) {
       const u64 y = Yq[HB1_RS * r];
       u64 v = nored ? y : y - __umul64hi(y, P.one_s) * P.q;   // y < 7 q_t as it is, or y mod q_t in [0, 2 q_t)
       if (y > qs_half) v += adj;                  // balanced representative: subtract q_s   -> below 8 q_t: fine for the CT network
       a[r] = v;
-    }
+    });
     {
       Hb1TwPtr tw;
       tw.p[0] = P.fw + 1; tw.p[1] = P.fw + 2; tw.p[2] = P.fw + 4; tw.p[3] = P.fw + 8;
       hb1_r16_fwd<SP>(a, tw, M);
     }
     hb_group_sync(grp, 64);   // the previous item's pass-2 reads of Wg are complete
-#pragma unroll
-    for (int r = 0; r < 16; r++) Wg[HB1_RS * r + x] = a[r];
+    hb1_unroll<16>([&](auto r) { Wg[HB1_RS * r + x] = a[r]; });
     hb_group_sync(grp, 64);
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = Wg[HB1_RS * x + l];
+    hb1_unroll<16>([&](auto l) { a[l] = Wg[HB1_RS * x + l]; });
     {
       Hb1TwPtr tw;
       tw.p[0] = P.fw + 16 + x; tw.p[1] = P.fw + 32 + 2 * x; tw.p[2] = P.fw + 64 + 4 * x; tw.p[3] = P.fw + 128 + 8 * x;
       hb1_r16_fwd<SP>(a, tw, M);
     }
     u64* d = dst + ((size_t)pi << J.logN) + c0 + 4 * qd + c;
-#pragma unroll
-    for (int l = 0; l < 16; l++) d[(size_t)(16 * x + l) << 8] = a[l];   // lazy: k1_fwd_blk finishes the transform
+    hb1_unroll<16>([&](auto l) { d[(size_t)(16 * x + l) << 8] = a[l]; });   // lazy: k1_fwd_blk finishes the transform
   }
 }
 

@@ -22,9 +22,8 @@
 //     16 resident compute warps per SM as two 9-warp CTAs, but 112 registers per thread instead of 96 (register
 //     allocation rounds a 288-thread CTA up to 320).
 //
-// Measured on an H100 SXM (80 GB HBM3, 400 W limit), alternated in one run: both kernels are slower than k1_fwd_blk / k1_inv_blk
-// (6.06 against 5.30 ms per mod-down launch of the multiply benchmark forward, 2.01 against 1.67 ms inverse; 1 515 against
-// 1 600 mult/s), so they run only with HB_BLK_V2=1.
+// Measured on an H100 SXM (80 GB HBM3, 400 W limit), two runs each in one session: both kernels together are slower than
+// k1_fwd_blk / k1_inv_blk (2 504-2 507 against 2 543-2 548 mult/s on the multiply benchmark), so they run only with HB_BLK_V2=1.
 //
 // smem per team (1024-byte aligned): IN[2][4096] | OUT[4096] | TW1[16][16] | 7 mbarriers  (101 KB; 203 KB per CTA)
 #pragma once
@@ -251,26 +250,19 @@ __global__ void __launch_bounds__(HB2_THREADS, 1) k2_fwd_blk(const HbPrimeDev* _
         const int g = e - ((1 << kk) - 1);
         TW1[j1 * 16 + e] = P.fw[((size_t)1 << (n1 + kk)) + ((size_t)b1 << kk) + g];
       }
-#pragma unroll
-      for (int kk = 0; kk < 4; kk++)
-#pragma unroll
-        for (int g = 0; g < (1 << kk); g++)
-          tw2.t[(1 << kk) - 1 + g] = P.fw[((size_t)1 << (n1 + 4 + kk)) + ((size_t)b2 << (4 + kk)) + ((size_t)hi << kk) + g];
+      tw2.load([&](int kk, int g) { return P.fw[((size_t)1 << (n1 + 4 + kk)) + ((size_t)b2 << (4 + kk)) + ((size_t)hi << kk) + g]; });
       __syncwarp();
     }
     const bool e = epi1 || (epi3 && sc != 0);
     u64* T = IN + (k & 1) * HB2_TILE;
     hb2_mbar_wait(BAR + HB2_FULL0 + (k & 1), (unsigned)(k >> 1) & 1u);
     u64 a[16];
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = T[p1 + 16 * r + lo];
+    hb1_unroll<16>([&](auto r) { a[r] = T[p1 + 16 * r + lo]; });
     hb1_r16_fwd<SP>(a, tw1, M);
     __syncwarp();   // every lane holds its inputs: the block may be overwritten
-#pragma unroll
-    for (int r = 0; r < 16; r++) T[p1 + 16 * r + (x1 ^ r)] = a[r];
+    hb1_unroll<16>([&](auto r) { T[p1 + 16 * r + (x1 ^ r)] = a[r]; });
     __syncwarp();
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = T[p2 + (x2 ^ l)];
+    hb1_unroll<16>([&](auto l) { a[l] = T[p2 + (x2 ^ l)]; });
     hb2_fence_async();   // the in-place exchange wrote the slot through the generic proxy; the refill is an async-proxy write
     __syncwarp();
     if (lane == 0) hb2_mbar_arrive(BAR + HB2_EMPTY0 + (k & 1));   // the slot can be refilled
@@ -278,13 +270,12 @@ __global__ void __launch_bounds__(HB2_THREADS, 1) k2_fwd_blk(const HbPrimeDev* _
     hb2_mbar_wait(BAR + HB2_OUTFREE, pfree); pfree ^= 1u;
     if (e) {
       hb2_mbar_wait(BAR + HB2_OLDFULL, pold); pold ^= 1u;
-#pragma unroll
-      for (int l = 0; l < 16; l++) {
+      hb1_unroll<16>([&](auto l) {
         u64* o = OUT + po + 256 * (int)hb1_brev4((unsigned)l);
         u64 v = hb1_shoup4<SP>(*o - a[l] + (M.qb2 + M.qb), sc, sc_s, M);   // (old - x) * scal, x in [0, 8q + 2^32), old < 4q
         if (!lazy) v = hb1_canon4(v, q);
         *o = v;
-      }
+      });
       if (epi3) {   // two stores from one buffer: the updated matrix first, then x itself
         hb2_fence_async();
         __syncwarp();
@@ -293,8 +284,7 @@ __global__ void __launch_bounds__(HB2_THREADS, 1) k2_fwd_blk(const HbPrimeDev* _
       }
     }
     if (!epi1) {
-#pragma unroll
-      for (int l = 0; l < 16; l++) OUT[po + 256 * (int)hb1_brev4((unsigned)l)] = lazy ? a[l] : hb1_canon_fwd(a[l], q, M.qb);
+      hb1_unroll<16>([&](auto l) { OUT[po + 256 * (int)hb1_brev4((unsigned)l)] = lazy ? a[l] : hb1_canon_fwd(a[l], q, M.qb); });
     }
     hb2_fence_async();
     __syncwarp();
@@ -372,18 +362,13 @@ __global__ void __launch_bounds__(HB2_THREADS, 1) k2_inv_blk(const HbPrimeDev* _
         const int g = e - ((1 << kk) - 1);
         TW1[j1 * 16 + e] = P.iw[((size_t)1 << (n1 + kk)) + ((size_t)b1 << kk) + g];
       }
-#pragma unroll
-      for (int kk = 0; kk < 4; kk++)
-#pragma unroll
-        for (int g = 0; g < (1 << kk); g++)
-          tw2.t[(1 << kk) - 1 + g] = P.iw[((size_t)1 << (n1 + 4 + kk)) + ((size_t)b2 << (4 + kk)) + ((size_t)hi << kk) + g];
+      tw2.load([&](int kk, int g) { return P.iw[((size_t)1 << (n1 + 4 + kk)) + ((size_t)b2 << (4 + kk)) + ((size_t)hi << kk) + g]; });
       __syncwarp();
     }
     const u64* T = IN + (k & 1) * HB2_TILE;
     hb2_mbar_wait(BAR + HB2_FULL0 + (k & 1), (unsigned)(k >> 1) & 1u);
     u64 a[16];
-#pragma unroll
-    for (int l = 0; l < 16; l++) a[l] = T[po + 256 * (int)hb1_brev4((unsigned)l)];
+    hb1_unroll<16>([&](auto l) { a[l] = T[po + 256 * (int)hb1_brev4((unsigned)l)]; });
     __syncwarp();
     if (lane == 0) hb2_mbar_arrive(BAR + HB2_EMPTY0 + (k & 1));
     hb1_r16_inv<SP>(a, tw2, M);
@@ -391,15 +376,12 @@ __global__ void __launch_bounds__(HB2_THREADS, 1) k2_inv_blk(const HbPrimeDev* _
     // warp's own previous store has to be done reading them
     if (lane == 0) hb2_store_wait_read();
     __syncwarp();
-#pragma unroll
-    for (int l = 0; l < 16; l++) OUT[p2 + (x2 ^ l)] = a[l];
+    hb1_unroll<16>([&](auto l) { OUT[p2 + (x2 ^ l)] = a[l]; });
     __syncwarp();
-#pragma unroll
-    for (int r = 0; r < 16; r++) a[r] = OUT[p1 + 16 * r + (x1 ^ r)];
+    hb1_unroll<16>([&](auto r) { a[r] = OUT[p1 + 16 * r + (x1 ^ r)]; });
     hb1_r16_inv<SP>(a, tw1, M);
     __syncwarp();   // all swizzled reads done before the dense results land
-#pragma unroll
-    for (int r = 0; r < 16; r++) OUT[p1 + 16 * r + lo] = J.epi == 2 ? a[r] : hb1_canon_inv(a[r], q);
+    hb1_unroll<16>([&](auto r) { OUT[p1 + 16 * r + lo] = J.epi == 2 ? a[r] : hb1_canon_inv(a[r], q); });
     hb2_fence_async();
     __syncwarp();
     if (lane == 0) {   // block b = slot*G + brev(ug) of the row, 2 KB contiguous each
