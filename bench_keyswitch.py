@@ -7,6 +7,10 @@
   --mode replicas : independent ciphertexts per GPU, evk replicated, no collective.  scaling = "weak".
                     BASELINE config 3 (BGV m=2^17 p=257 bits=1500 c=3) by default.
 
+  --prg           : instead, the device expansion of key-switching rows from a PRG seed (hb_poly_randomize):
+                    all a_i of a config-3 matrix (3 x 35 rows, N = 2^16) and of config 2's, ms per matrix over
+                    repeated runs, GB/s of key stream consumed, the count and fill passes separately.
+
 Launch: python bench_keyswitch.py [--mode ...]            (1 GPU)
         python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench_keyswitch.py --gpus N ...
 Prints one JSON line on rank 0 (key-switches/s = 3-part -> 2-part over S|special, then mod-down to S).
@@ -24,6 +28,58 @@ WORKLOADS = {
     "cfg3": {"name": "bgv_m2^17_p257_bits1500_c3 (l=26,K=9,d=3)", "m": 1 << 17, "p": 257, "r": 1, "bits": 1500, "c": 3},
 }
 ROW = (1 << 16) * 8
+PRG_WORKLOADS = {
+    "cfg3": {"name": "bgv_m2^17_p257_bits1500_c3", "m": 1 << 17, "p": 257, "r": 1, "bits": 1500, "c": 3},
+    "cfg2": {"name": "ckks_m2^17_bits1190_c2", "m": 1 << 17, "p": -1, "r": 1, "bits": 1190, "c": 2},
+}
+PRG_SEED = 0xB7E151628AED2A6ABF7158809CF4F3C762E7160F38B4DA56A784D9045190CFEF
+
+
+def bench_prg(args):
+    """ms per key-switching matrix expanded from its seed: SetSeed(prgSeed); a[i].randomize() for every digit i over
+    ctxt|special, one hb_poly_randomize call.  The rows are checked against the vectorised oracle, which also gives the
+    exact number of 2048-byte key-stream buffers the matrix consumes."""
+    import numpy as np
+    sys.path.insert(0, os.path.join(ROOT, "oracle"))
+    import ntl_prg_np as npg
+    from bench import gpu_identity
+    from helib_b200 import Chain, Engine
+    out = {"metric": "prg_matrix_expansion", "unit": "ms/matrix", "gpu": gpu_identity(0), "steps": args.steps, "reps": args.reps, "workloads": []}
+    for key, wl in PRG_WORKLOADS.items():
+        ch = Chain(wl["m"], wl["p"], wl["r"], wl["bits"], wl["c"])
+        E = Engine(wl["m"], ch.primes, None, ch.digits, ch.special)
+        full = ch.ctxt + ch.special
+        n = len(ch.digits)
+        A = [E.poly() for _ in range(n)]
+        E.randomize(A, full, PRG_SEED)
+        bs = npg.BufferStream(PRG_SEED)
+        for d in range(n):
+            ref = npg.randomize_rows(ch.primes, E.N, full, bs)
+            got = A[d].download(full)
+            assert all(np.array_equal(got[i], ref[i]) for i in full), f"{key}: device rows differ from the oracle"
+        stream_bytes = bs.next * 2048
+        for _ in range(max(1, args.warmup)):
+            E.randomize(A, full, PRG_SEED)
+        runs = []
+        for _ in range(args.reps):
+            E.mark_begin()
+            for _ in range(args.steps):
+                E.randomize(A, full, PRG_SEED)
+            runs.append(E.mark_end() / args.steps)
+        E.profile(True)
+        E.randomize(A, full, PRG_SEED)
+        E.profile(False)
+        prof = {r["kernel"]: {"launches": r["launches"], "ms": round(r["ms"], 4)} for r in E.profile_results()}
+        med = float(np.median(runs))
+        out["workloads"].append({
+            "workload": wl["name"], "N": E.N, "polys": n, "rows_per_poly": len(full),
+            "key_stream_MB": round(stream_bytes / 1e6, 2),
+            "ms_per_matrix": {"median": round(med, 4), "min": round(min(runs), 4), "max": round(max(runs), 4)},
+            "key_stream_GBps": round(stream_bytes / (med / 1e3) / 1e9, 1),
+            "passes": prof,
+        })
+        E.close()
+    print(json.dumps(out))
 
 
 def main():
@@ -37,7 +93,11 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="do not capture the step into a CUDA graph")
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "gather"], help="sharded mode: peer stores from the producing kernel, or pack/all_gather/unpack")
     ap.add_argument("--profile", action="store_true", help="add a per-kernel table (CUDA events per launch, one eager step)")
+    ap.add_argument("--prg", action="store_true", help="time the device expansion of key-switching rows from a PRG seed instead")
+    ap.add_argument("--reps", type=int, default=5, help="--prg: timed runs of --steps expansions each")
     args = ap.parse_args()
+    if args.prg:
+        return bench_prg(args)
     import numpy as np
     import torch
     import torch.distributed as dist

@@ -7,7 +7,7 @@ import subprocess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["csrc/hb_engine.cu", "csrc/hb_chain.cpp"]
-DEPS = ["csrc/hb_engine.cu", "csrc/hb_device.cuh", "csrc/hb_device_v1.cuh", "csrc/hb_device_v2.cuh", "csrc/hb_device_gen.cuh", "csrc/hb_chain.cpp", "../include/helib_b200.h", "../include/helib_b200_chain.h"]
+DEPS = ["csrc/hb_engine.cu", "csrc/hb_device.cuh", "csrc/hb_device_v1.cuh", "csrc/hb_device_v2.cuh", "csrc/hb_device_gen.cuh", "csrc/hb_device_prg.cuh", "csrc/hb_chain.cpp", "../include/helib_b200.h", "../include/helib_b200_chain.h"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 

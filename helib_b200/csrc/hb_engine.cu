@@ -7,6 +7,7 @@
 #include "hb_device_v1.cuh"
 #include "hb_device_v2.cuh"
 #include "hb_device_gen.cuh"
+#include "hb_device_prg.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -113,6 +114,10 @@ struct hb_ctx {
   std::vector<ProfRec> prof_pending;
   struct ProfAgg { std::string name; u64 launches; double ms; u64 bytes; };
   std::vector<ProfAgg> prof;
+  // seeded row expansion (hb_poly_randomize): row starts, per-buffer offsets and the CTA ticket of k_prg_count
+  u64* prg_start = nullptr; unsigned* prg_off = nullptr; unsigned long long* prg_ticket = nullptr;
+  size_t prg_start_cap = 0, prg_off_cap = 0;
+  int prg_window = 0;   // HB_PRG_WINDOW=w: count w buffers per row in parallel instead of the statistical bound (tests the slow path)
 };
 struct hb_poly { hb_ctx* ctx; u64* d; bool owned = true; bool ipc = false; };
 
@@ -204,6 +209,7 @@ static int ctx_build(hb_ctx* c, hb_ctx** out, int device, uint64_t m, int nprime
   { const char* e = getenv("HB_CONV1"); c->conv1 = !(e && e[0] == '0'); }
   { const char* e = getenv("HB_BLK_V2"); c->blk_v2 = e && e[0] == '1'; }
   { const char* e = getenv("HB_CHUNK"); int v = e ? atoi(e) : HB_MAXB; c->chunk = v >= 1 && v <= HB_MAXB ? v : HB_MAXB; }
+  { const char* e = getenv("HB_PRG_WINDOW"); int v = e ? atoi(e) : 0; c->prg_window = v >= 1 ? v : 0; }
   c->resident_ctas = 264;   // 2 per SM on a 132-SM H100 if the device query fails
 #ifdef HB_SIM
   c->resident_ctas = 7;   // few, odd: every simulated CTA walks several units and crosses (row, block-group) boundaries
@@ -323,6 +329,7 @@ extern "C" void hb_ctx_destroy(hb_ctx* c) {
   cudaFree(c->gen.d_W);
   cudaFree(c->gen.w0); cudaFree(c->gen.w1); cudaFree(c->gen.wt); cudaFree(c->gen.cA); cudaFree(c->gen.cB);
   cudaFree(c->tmpA); cudaFree(c->tmpB); cudaFree(c->d_tw); cudaFree(c->d_primes); cudaFree(c->d_stats);
+  cudaFree(c->prg_start); cudaFree(c->prg_off); cudaFree(c->prg_ticket);
   for (HbTmap* sl : c->tmap_slabs) cudaFree(sl);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
   delete c;
@@ -552,6 +559,70 @@ extern "C" int hb_poly_deserialize(hb_poly* p, const void* buf, uint64_t buflen,
   *n_out = (int)card;
   return HB_OK;
 }
+
+// ---- seeded expansion: SetSeed(seed); for p in polys: p.randomize() over rows idx (src/DoubleCRT.cpp:1258-1378) =====
+static int prg_grow(hb_ctx* c, void** p, size_t* cap, size_t bytes) {
+  if (*cap >= bytes) return HB_OK;
+  if (*p) { HB_CUDA(cudaFree(*p)); c->bytes -= *cap; *p = nullptr; *cap = 0; }   // cudaFree waits for the kernels using it
+  HB_TRY(ctx_alloc(c, p, bytes));
+  *cap = bytes;
+  return HB_OK;
+}
+extern "C" int hb_poly_randomize(hb_poly* const* polys, int npolys, const int32_t* idx, int n, const uint8_t* seed, int seedlen) {
+  static const char* who = "hb_poly_randomize";
+  if (!polys || npolys <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: no polynomials", who);
+  if (seedlen < 0 || (seedlen > 0 && !seed)) return hb_fail(HB_ERR_BAD_ARG, "%s: null seed with length %d", who, seedlen);
+  hb_ctx* c = nullptr;
+  HB_TRY(check_polys(polys, npolys, &c, who));
+  HB_TRY(check_idx(c, idx, n, who, true));
+  for (int i = 1; i < n; i++) if (idx[i] <= idx[i - 1]) return hb_fail(HB_ERR_BAD_ARG, "%s: prime indices must be strictly ascending", who);
+  if (n == 0) return HB_OK;
+  const HbPrgKey key = hb_prg_derive_key(seed, seedlen);
+  const u64 N = c->N;
+  const int T = npolys * n;
+  std::vector<HbPrgRow> rows((size_t)T);
+  int wmax = 1;
+  for (int r = 0; r < n; r++) {
+    const u64 q = c->q[idx[r]];
+    const int k = h_bitlen(q - 1), nb = (k + 7) / 8;
+    const int w = c->prg_window ? c->prg_window : hb_prg_window(q, k, nb, N);
+    wmax = std::max(wmax, w);
+    for (int p = 0; p < npolys; p++) {
+      HbPrgRow& R = rows[(size_t)p * n + r];
+      R.q = q; R.mask = k >= 64 ? ~0ULL : (1ULL << k) - 1; R.nb = nb; R.window = w;
+      R.row = polys[p]->d + (size_t)idx[r] * N;
+    }
+  }
+  HB_TRY(prg_grow(c, (void**)&c->prg_start, &c->prg_start_cap, (size_t)(T + 1) * sizeof(u64)));
+  HB_TRY(prg_grow(c, (void**)&c->prg_off, &c->prg_off_cap, (size_t)T * wmax * sizeof(unsigned)));
+  if (!c->prg_ticket) {
+    HB_TRY(ctx_alloc(c, (void**)&c->prg_ticket, sizeof(unsigned long long)));
+    HB_CUDA(cudaMemsetAsync(c->prg_ticket, 0, sizeof(unsigned long long), c->stream));
+  }
+  HB_CUDA(cudaMemsetAsync(c->prg_start, 0, sizeof(u64), c->stream));   // a fresh SetSeed: the first row starts at buffer 0
+  // the row chain: each launch reads its row's first buffer from device memory and writes the next row's
+  HbPrgCountJob C;
+  C.key = key; C.N = N; C.start = c->prg_start; C.ticket = c->prg_ticket;
+  for (int t = 0; t < T; t++) {
+    C.r = rows[(size_t)t]; C.t = t; C.off = c->prg_off + (size_t)t * wmax;
+    pre_launch(c);
+    HB_LAUNCH(k_prg_count, dim3((unsigned)((C.r.window + HB_PRG_WARPS - 1) / HB_PRG_WARPS)), dim3(HB_PRG_THREADS), HB_PRG_SMEM_BYTES, c->stream, C);
+    HB_TRY(post_launch(c, "k_prg_count", (u64)C.r.window * sizeof(unsigned) * 2));
+  }
+  // every (row, buffer) at once
+  HbPrgFillJob F;
+  F.key = key; F.N = N; F.start = c->prg_start; F.off = c->prg_off; F.wmax = wmax;
+  for (int t0 = 0; t0 < T; t0 += HB_PRG_MAXT) {
+    const int nt = std::min(HB_PRG_MAXT, T - t0);
+    F.t0 = t0;
+    for (int i = 0; i < nt; i++) F.r[i] = rows[(size_t)t0 + i];
+    pre_launch(c);
+    HB_LAUNCH(k_prg_fill, dim3((unsigned)((wmax + HB_PRG_WARPS - 1) / HB_PRG_WARPS), (unsigned)nt), dim3(HB_PRG_THREADS), HB_PRG_SMEM_BYTES, c->stream, F);
+    HB_TRY(post_launch(c, "k_prg_fill", (u64)nt * N * 8));
+  }
+  return HB_OK;
+}
+
 static int pool_get(hb_ctx* c, int n, std::vector<hb_poly*>& out) {
   while ((int)c->pool.size() < n) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->pool.push_back(p); }
   out.assign(c->pool.begin(), c->pool.begin() + n);

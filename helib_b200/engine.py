@@ -346,6 +346,18 @@ class Engine:
         self._ck(self.lib.hb_mul_relin_moddown(_arr(a0), _arr(a1), _arr(b0), _arr(b1), len(a0), pi, ni, ps, ns,
                                                C.c_uint64(int(ptxt_space)), _arr(evk_a), _arr(evk_b), len(evk_a)))
 
+    def randomize(self, polys, idx, seed):
+        """NTL::SetSeed(seed), then p.randomize() over rows idx for each p in polys, expanded on the device
+        (hb_poly_randomize).  seed: the ZZ's little-endian magnitude bytes, or a non-negative int."""
+        if isinstance(seed, int):
+            if seed < 0:
+                raise ValueError("seed must be non-negative")
+            seed = seed.to_bytes((seed.bit_length() + 7) // 8, "little")
+        seed = bytes(seed)
+        a, p, n = _idx(idx)
+        buf = (C.c_uint8 * max(1, len(seed))).from_buffer_copy(seed or b"\0")
+        self._ck(self.lib.hb_poly_randomize(_arr(polys), len(polys), p, n, buf, len(seed)))
+
 
 class Chain:
     """Host-side prime chain (hb_chain): helib::Context::buildModChain reproduced in C++."""

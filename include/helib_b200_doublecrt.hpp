@@ -22,6 +22,7 @@
 #include <chrono>
 #include <map>
 #include <mutex>
+#include <type_traits>
 
 #include "helib_b200.h"
 #include "helib_b200_chain.h"
@@ -395,7 +396,8 @@ class DoubleCRT {
   // get(buf, 2048) stands for NTL::RandomStream::get (the ChaCha20 stream keyed by SetSeed; not restated).  A fresh 2048-byte
   // buffer per refill and per row, nb = ceil(bits(q-1)/8) little-endian bytes per candidate, masked, accepted when < q.
   // Runs on the host (once per key-switching matrix) and uploads the rows.
-  template <class GetBytes> void randomize(GetBytes&& get) {
+  template <class GetBytes, std::enable_if_t<!std::is_same<std::decay_t<GetBytes>, std::vector<uint8_t>>::value, int> = 0>
+  void randomize(GetBytes&& get) {
     const long N = context_->getPhiM(), bufsz = 2048;
     std::vector<uint64_t> dense((size_t)context_->numPrimes() * N, 0);
     std::vector<unsigned char> buf((size_t)bufsz);
@@ -420,6 +422,13 @@ class DoubleCRT {
     auto idx = set_.vec();
     if (!idx.empty()) check(hb_poly_upload(p_, idx.data(), (int)idx.size(), dense.data()));
     check(hb_ctx_sync(context_->handle()));
+  }
+  // randomize(&seed) (src/DoubleCRT.cpp:1258-1378 after NTL::SetSeed(seed)): the same rows from NTL's own stream, expanded
+  // on the device.  seed = the little-endian magnitude bytes of the ZZ (high-order zero bytes do not count; empty = 0).
+  void randomize(const std::vector<uint8_t>& seed) {
+    auto idx = set_.vec();
+    hb_poly* d[1] = {p_};
+    if (!idx.empty()) check(hb_poly_randomize(d, 1, idx.data(), (int)idx.size(), seed.data(), (int)seed.size()));
   }
   // toPoly (src/DoubleCRT.cpp:925-1113): N x L little-endian two's-complement limbs
   std::vector<uint64_t> toPoly(const IndexSet& s, bool positive, int& L) const {
