@@ -10,6 +10,11 @@
   --prg           : instead, the device expansion of key-switching rows from a PRG seed (hb_poly_randomize):
                     all a_i of a config-3 matrix (3 x 35 rows, N = 2^16) and of config 2's, ms per matrix over
                     repeated runs, GB/s of key stream consumed, the count and fill passes separately.
+  --seeded        : instead, key-switching matrices held as b_i plus their PRG seed (hb_poly_create_seeded: every key
+                    switch regenerates the a_i rows it reads) against the same matrices expanded, alternated in one
+                    process: config-3 relinearise + mod-down in groups of 64, config-2 multiply + relinearise + mod-down
+                    at batch 32, and hoisted rotations on config 5's ring (m = 21845) at batch 8 with one matrix per
+                    amount.  Both rates, an in-run bit-identity check, device bytes per matrix and creation time.
 
 Launch: python bench_keyswitch.py [--mode ...]            (1 GPU)
         python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench_keyswitch.py --gpus N ...
@@ -82,6 +87,143 @@ def bench_prg(args):
     print(json.dumps(out))
 
 
+SEEDED_WORKLOADS = {
+    "cfg3_relin_moddown": {"name": "bgv_m2^17_p257_bits1500_c3 relinearize+scale_down", "m": 1 << 17, "p": 257, "bits": 1500, "c": 3, "batch": 64},
+    "cfg2_mul_relin_moddown": {"name": "ckks_m2^17_bits1190_c2 mul_relin_moddown", "m": 1 << 17, "p": -1, "bits": 1190, "c": 2, "batch": 32},
+    "cfg5_hoisted_rotation": {"name": "bgv_m21845_p2_bits580_c2_bootstrappable automorph_keyswitch_digits", "m": 21845, "p": 2, "bits": 580, "c": 2,
+                              "batch": 8, "bootstrappable": True, "amounts": 4},
+}
+
+
+def _seeded_workload(args, key, wl, ch, E):
+    import time
+    import numpy as np
+    N, npr, B = E.N, E.np, wl["batch"]
+    p = 1 if ch.p == -1 else ch.p
+    S = ch.ctxt
+    full = sorted(ch.ctxt + ch.special)
+    nd = len(ch.digits)
+    rng = np.random.Generator(np.random.Philox(20261015))
+
+    def rand(idx):
+        x = np.zeros((npr, N), dtype=np.uint64)
+        for i in idx:
+            x[i] = rng.integers(0, ch.primes[i], size=N, dtype=np.uint64)
+        return x
+
+    nkeys = wl.get("amounts", 1)
+    seeds = [PRG_SEED + j for j in range(nkeys)]
+    b0 = E.stats()["device_bytes"]
+    EA = [[E.poly() for _ in range(nd)] for _ in range(nkeys)]
+    expanded_bytes = (E.stats()["device_bytes"] - b0) // nkeys
+    for A, sd in zip(EA, seeds):
+        E.randomize(A, full, sd)
+    E.sync()
+    b1 = E.stats()["device_bytes"]
+    SA = [E.seeded(nd, full, sd) for sd in seeds]
+    seeded_bytes = (E.stats()["device_bytes"] - b1) // nkeys
+    create_ms = []
+    for _ in range(5):
+        E.sync()
+        t0 = time.perf_counter()
+        tmp = E.seeded(nd, full, PRG_SEED)
+        E.sync()
+        create_ms.append((time.perf_counter() - t0) * 1e3)
+        del tmp
+    EB = [[E.poly(rand(full), full) for _ in range(nd)] for _ in range(nkeys)]
+
+    if key == "cfg3_relin_moddown":
+        Sp = full
+        src = [[rand(S) for _ in range(3)] for _ in range(B)]
+        C = [[E.poly(x[k], S) for k in range(3)] for x in src]
+        C0, C1, C2 = ([c[k] for c in C] for k in range(3))
+
+        def load():
+            for c, x in zip(C, src):
+                for k in range(3):
+                    c[k].upload(x[k], S)
+
+        def step(A, j=0):
+            E.relinearize(C0, C1, C2, S, A[0], EB[0])
+            E.scale_down(C0 + C1, Sp, S, p)
+        outputs, out_idx = (lambda: C0 + C1), S
+    elif key == "cfg2_mul_relin_moddown":
+        S_in, S = ch.ctxt, ch.ctxt[:-1]
+        src = [[rand(S_in) for _ in range(4)] for _ in range(B)]
+        P = [[E.poly(x[k], S_in) for k in range(4)] for x in src]
+        A0, A1, B0, B1 = ([q[k] for q in P] for k in range(4))
+
+        def load():
+            for q, x in zip(P, src):
+                for k in range(4):
+                    q[k].upload(x[k], S_in)
+
+        def step(A, j=0):
+            E.mul_relin_moddown(A0, A1, B0, B1, S_in, S, p, A[0], EB[0])
+        outputs, out_idx = (lambda: A0 + A1), S
+    else:
+        Sp = full
+        C0 = [E.poly(rand(S), S) for _ in range(B)]
+        digs = E.break_into_digits([E.poly(rand(S), S) for _ in range(B)], S)
+        O0, O1 = [E.poly() for _ in range(B)], [E.poly() for _ in range(B)]
+        amounts = [t for t in range(2, wl["m"]) if np.gcd(t, wl["m"]) == 1][:nkeys]
+
+        def load():
+            pass
+
+        def step(A, j=None):
+            for a in (range(nkeys) if j is None else [j]):
+                E.automorph_keyswitch_digits(digs, S, C0, amounts[a], A[a], EB[a], O0, O1)
+        outputs, out_idx = (lambda: O0 + O1), Sp
+
+    # in-run check: the same inputs through both forms give the same output rows
+    got = []
+    for A in (EA, SA):
+        load()
+        step(A, 0) if key == "cfg5_hoisted_rotation" else step(A)
+        got.append([x.download(out_idx)[out_idx] for x in outputs()])
+    identical = all(np.array_equal(a, b) for a, b in zip(*got))
+    per_call = nkeys if key == "cfg5_hoisted_rotation" else 1
+    runs = {"expanded": [], "seeded": []}
+    for form, A in (("expanded", EA), ("seeded", SA)):
+        for _ in range(max(1, args.warmup)):
+            step(A)
+    for _ in range(args.reps):
+        for form, A in (("expanded", EA), ("seeded", SA)):
+            E.sync()
+            E.mark_begin()
+            for _ in range(args.steps):
+                step(A)
+            ms = E.mark_end() / (args.steps * per_call)
+            runs[form].append(B / (ms / 1e3))
+    med = {f: float(np.median(v)) for f, v in runs.items()}
+    return {
+        "workload": wl["name"], "N": N, "batch": B, "digits": nd, "rows_per_a": len(full), "matrices": nkeys,
+        "rate_items_per_s": {f: {"median": round(med[f], 1), "min": round(min(v), 1), "max": round(max(v), 1)} for f, v in runs.items()},
+        "seeded_vs_expanded": round(med["seeded"] / med["expanded"] - 1.0, 4),
+        "outputs_bit_identical": identical,
+        "device_bytes_per_matrix_a": {"expanded": expanded_bytes, "seeded": seeded_bytes},
+        "device_bytes_per_matrix_a_and_b": {"expanded": 2 * expanded_bytes, "seeded": expanded_bytes + seeded_bytes},
+        "create_seeded_ms": {"median": round(float(np.median(create_ms)), 3), "min": round(min(create_ms), 3)},
+    }
+
+
+def bench_seeded(args):
+    """Expanded against seeded a_i in the key-switching entry points, alternated run by run in one process."""
+    from bench import gpu_identity
+    from helib_b200 import Chain, Engine
+    out = {"metric": "seeded_keyswitch_matrices", "unit": "items/s", "gpu": gpu_identity(0), "steps": args.steps, "reps": args.reps,
+           "workloads": []}
+    for key, wl in SEEDED_WORKLOADS.items():
+        ch = Chain(wl["m"], wl["p"], 1, wl["bits"], wl["c"], bootstrappable=wl.get("bootstrappable", False))
+        E = Engine(wl["m"], ch.primes, None, ch.digits, ch.special)
+        out["workloads"].append(_seeded_workload(args, key, wl, ch, E))   # its polys are freed on return
+        E.close()
+    print(json.dumps(out))
+    if not all(w["outputs_bit_identical"] for w in out["workloads"]):
+        sys.exit(1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -94,10 +236,13 @@ def main():
     ap.add_argument("--exchange", default="p2p", choices=["p2p", "gather"], help="sharded mode: peer stores from the producing kernel, or pack/all_gather/unpack")
     ap.add_argument("--profile", action="store_true", help="add a per-kernel table (CUDA events per launch, one eager step)")
     ap.add_argument("--prg", action="store_true", help="time the device expansion of key-switching rows from a PRG seed instead")
-    ap.add_argument("--reps", type=int, default=5, help="--prg: timed runs of --steps expansions each")
+    ap.add_argument("--reps", type=int, default=5, help="--prg: timed runs of --steps expansions each; --seeded: runs of each form")
+    ap.add_argument("--seeded", action="store_true", help="time key switches with seeded against expanded a_i instead")
     args = ap.parse_args()
     if args.prg:
         return bench_prg(args)
+    if args.seeded:
+        return bench_seeded(args)
     import numpy as np
     import torch
     import torch.distributed as dist

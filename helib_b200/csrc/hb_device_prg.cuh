@@ -14,7 +14,8 @@
 //                per-buffer row offsets and writes B_{t+1} to device memory, which the next launch reads.  A row that
 //                needs more than window_t buffers is finished by that CTA itself, 8 buffers at a time (slow path).
 //   k_prg_fill   one launch over all (row, buffer): regenerates each buffer, compacts its accepted candidates with a
-//                ballot prefix sum and writes them to row[offset + rank] for positions < N.
+//                ballot prefix sum and writes them to row[offset + rank] for positions < N.  Each launch row names the
+//                schedule row it reads, so a kept schedule (hb_poly_create_seeded) refills any subset of its rows later.
 // A warp makes one buffer, one 64-byte block per lane; the ChaCha state stays in registers and the candidates are read
 // back through the warp's 2 KB slice of shared memory.
 #pragma once
@@ -65,7 +66,7 @@ struct HbPrgKey { unsigned k[8]; };   // the ChaCha20 key as little-endian words
 // one row of the expansion: prime, its candidate format and where its values go
 struct HbPrgRow {
   u64 q, mask;       // mask = 2^k - 1, k = bits(q-1)
-  u64* row;          // N residues
+  u64* row;          // N residues; nullptr in a count that only builds a schedule (hb_poly_create_seeded)
   int nb;            // bytes per candidate, ceil(k/8)
   int window;        // buffers counted in parallel for this row
 };
@@ -80,13 +81,15 @@ struct HbPrgCountJob {
   int t;
 };
 
+// launch row y fills r[y].row from schedule row sr[y]: any subset of a schedule's rows, in any order
 struct HbPrgFillJob {
   HbPrgKey key;
   u64 N;
   const u64* start;
-  const unsigned* off;             // row t's offsets at off + t*wmax
-  int t0, wmax;
+  const unsigned* off;             // schedule row s's offsets at off + s*wstride
+  int wstride;
   HbPrgRow r[HB_PRG_MAXT];
+  unsigned sr[HB_PRG_MAXT];
 };
 
 __device__ __forceinline__ unsigned hb_rotl32(unsigned x, int n) { return (x << n) | (x >> (32 - n)); }
@@ -206,7 +209,8 @@ __global__ void __launch_bounds__(HB_PRG_THREADS) k_prg_count(const HB_GRID_CONS
   __syncthreads();
   if (total >= N) return;   // block-uniform
 
-  // slow path: the window held fewer than N values; this CTA writes the rest of the row, 8 buffers per round
+  // slow path: the window held fewer than N values; this CTA writes the rest of the row, 8 buffers per round (or, when it
+  // only builds a schedule, just finds the next row's start)
   unsigned* wc = flag + 2;
   u64 base = total, b = B + W;
   while (base < N) {
@@ -216,7 +220,7 @@ __global__ void __launch_bounds__(HB_PRG_THREADS) k_prg_count(const HB_GRID_CONS
     __syncthreads();
     u64 pos = base, tot = 0;
     for (unsigned i = 0; i < HB_PRG_WARPS; i++) { if (i < warp) pos += wc[i]; tot += wc[i]; }
-    hb_prg_emit(buf, lane, J.r, pos, N, scr);
+    if (J.r.row) hb_prg_emit(buf, lane, J.r, pos, N, scr);   // grid-uniform
     if (lane == 0 && pos < N && pos + n >= N) J.start[J.t + 1] = b + warp + 1;
     __syncthreads();
     base += tot;
@@ -224,15 +228,15 @@ __global__ void __launch_bounds__(HB_PRG_THREADS) k_prg_count(const HB_GRID_CONS
   }
 }
 
-// grid = (ceil(wmax / 8), rows of this launch)
+// grid = (ceil(largest window / 8), rows of this launch)
 __global__ void __launch_bounds__(HB_PRG_THREADS) k_prg_fill(const HB_GRID_CONSTANT HbPrgFillJob J) {
   HB_SMEM_DECL
   const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const HbPrgRow& R = J.r[blockIdx.y];
   const unsigned w = blockIdx.x * HB_PRG_WARPS + warp;
   if (w >= (unsigned)R.window) return;   // warp-uniform; the kernel has no CTA barrier
-  const size_t t = (size_t)J.t0 + blockIdx.y;
-  const u64 pos = J.off[t * J.wmax + w];
+  const size_t t = J.sr[blockIdx.y];
+  const u64 pos = J.off[t * J.wstride + w];
   if (pos >= J.N) return;                 // past the buffer that completes the row
   u64* buf = HB_SMEM + warp * HB_PRG_WARP_SMEM;
   unsigned* scr = (unsigned*)(buf + HB_PRG_WORDS + 1);

@@ -118,8 +118,23 @@ struct hb_ctx {
   u64* prg_start = nullptr; unsigned* prg_off = nullptr; unsigned long long* prg_ticket = nullptr;
   size_t prg_start_cap = 0, prg_off_cap = 0;
   int prg_window = 0;   // HB_PRG_WINDOW=w: count w buffers per row in parallel instead of the statistical bound (tests the slow path)
+  std::vector<hb_poly*> ks_a;   // a_i regenerated from a seeded evk_a for the key switch in flight (allocated on first use)
 };
-struct hb_poly { hb_ctx* ctx; u64* d; bool owned = true; bool ipc = false; };
+// The row schedule of a seeded set (hb_poly_create_seeded): the ChaCha20 key, the rows, and in one device allocation the
+// first buffer of every schedule row (start[T+1]) and the exclusive row offset of every counted buffer (off[T*wmax]).
+// Schedule row p*n + r is row idx[r] of poly p.  Shared by the set's handles, freed with the last one.
+struct HbSeedSched {
+  HbPrgKey key;
+  std::vector<int32_t> idx;
+  std::vector<HbPrgRow> rows;   // per schedule row: candidate format and counted window (row pointers unset)
+  int wmax = 1;
+  void* blk = nullptr; size_t bytes = 0;
+  u64* start = nullptr; unsigned* off = nullptr;
+  int refs = 0;
+};
+// A seeded poly (sched != nullptr) has no rows: d is null.  Only the key-switching entry points (as evk_a) and hb_poly_expand
+// accept one; everything else rejects it before launching anything.
+struct hb_poly { hb_ctx* ctx; u64* d; bool owned = true; bool ipc = false; HbSeedSched* sched = nullptr; int sched_poly = 0; };
 
 static int ctx_alloc(hb_ctx* c, void** p, size_t bytes) {
   cudaError_t e = cudaMalloc(p, bytes);
@@ -330,6 +345,7 @@ extern "C" void hb_ctx_destroy(hb_ctx* c) {
   cudaFree(c->gen.w0); cudaFree(c->gen.w1); cudaFree(c->gen.wt); cudaFree(c->gen.cA); cudaFree(c->gen.cB);
   cudaFree(c->tmpA); cudaFree(c->tmpB); cudaFree(c->d_tw); cudaFree(c->d_primes); cudaFree(c->d_stats);
   cudaFree(c->prg_start); cudaFree(c->prg_off); cudaFree(c->prg_ticket);
+  for (hb_poly* p : c->ks_a) { cudaFree(p->d); delete p; }
   for (HbTmap* sl : c->tmap_slabs) cudaFree(sl);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
   delete c;
@@ -405,6 +421,11 @@ extern "C" int hb_poly_create(hb_ctx* c, hb_poly** out) {
 extern "C" void hb_poly_destroy(hb_poly* p) {
   if (!p) return;
   cudaStreamSynchronize(p->ctx->stream);
+  if (HbSeedSched* S = p->sched) {
+    if (--S->refs == 0) { if (S->blk) { cudaFree(S->blk); p->ctx->bytes -= S->bytes; } delete S; }
+    delete p;
+    return;
+  }
   if (p->owned) { p->ctx->bytes -= (size_t)p->ctx->nprimes * p->ctx->N * sizeof(u64); cudaFree(p->d); }
 #ifndef HB_SIM
   if (p->ipc) cudaIpcCloseMemHandle(p->d);
@@ -419,13 +440,20 @@ static int check_idx(hb_ctx* c, const int32_t* idx, int n, const char* who, bool
   }
   return HB_OK;
 }
-static int check_polys(hb_poly* const* p, int n, hb_ctx** c, const char* who) {
+// allow_seeded: the evk_a lists of the key-switching entry points, which regenerate seeded entries before any kernel reads them
+static int check_polys(hb_poly* const* p, int n, hb_ctx** c, const char* who, bool allow_seeded = false) {
   if (!p || n <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: no polynomials", who);
   for (int i = 0; i < n; i++) {
     if (!p[i]) return hb_fail(HB_ERR_BAD_ARG, "%s: null polynomial handle", who);
+    if (p[i]->sched && !allow_seeded) return hb_fail(HB_ERR_BAD_ARG, "%s: a seeded polynomial has no rows (only evk_a and hb_poly_expand take one)", who);
     if (*c == nullptr) { *c = p[i]->ctx; g_chunk = (*c)->chunk; }
     if (p[i]->ctx != *c) return hb_fail(HB_ERR_INDEX_SET, "%s: incompatible objects (different contexts)", who);  // src/DoubleCRT.cpp:222-223
   }
+  return HB_OK;
+}
+// single-poly calls that read or write p->d
+static int check_dense(hb_poly* p, const char* who) {
+  if (p->sched) return hb_fail(HB_ERR_BAD_ARG, "%s: a seeded polynomial has no rows (only evk_a and hb_poly_expand take one)", who);
   return HB_OK;
 }
 // rows <-> dense host matrix; runs of consecutive prime indices (the usual case: a prime set is an interval,
@@ -443,12 +471,14 @@ static int copy_rows(hb_ctx* c, u64* dev, u64* host, const int32_t* idx, int n, 
 }
 extern "C" int hb_poly_upload(hb_poly* p, const int32_t* idx, int n, const uint64_t* host) {
   if (!p || !host) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_upload: null");
+  HB_TRY(check_dense(p, "hb_poly_upload"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_poly_upload"));
   return copy_rows(c, p->d, (u64*)host, idx, n, true);
 }
 extern "C" int hb_poly_download(hb_poly* p, const int32_t* idx, int n, uint64_t* host) {
   if (!p || !host) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_download: null");
+  HB_TRY(check_dense(p, "hb_poly_download"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_poly_download"));
   HB_TRY(copy_rows(c, p->d, (u64*)host, idx, n, false));
@@ -457,6 +487,7 @@ extern "C" int hb_poly_download(hb_poly* p, const int32_t* idx, int n, uint64_t*
 }
 extern "C" int hb_poly_download_async(hb_poly* p, const int32_t* idx, int n, uint64_t* host) {
   if (!p || !host) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_download_async: null");
+  HB_TRY(check_dense(p, "hb_poly_download_async"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_poly_download_async"));
   HB_TRY(copy_rows(c, p->d, (u64*)host, idx, n, false));
@@ -501,11 +532,13 @@ extern "C" int hb_ctx_profile_get(hb_ctx* c, int i, char* name, int namelen, uin
 // write_ntl_vec_long (int32 length, int32 intSize = 8, then little-endian int64 values; src/binio.cpp:103-122).
 extern "C" int hb_poly_serialized_size(hb_poly* p, int n, uint64_t* bytes) {
   if (!p || !bytes || n < 0) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_serialized_size: bad argument");
+  HB_TRY(check_dense(p, "hb_poly_serialized_size"));
   *bytes = 8 + 8ULL * n + (uint64_t)n * (8 + 8ULL * p->ctx->N);
   return HB_OK;
 }
 extern "C" int hb_poly_serialize(hb_poly* p, const int32_t* idx, int n, void* buf, uint64_t buflen) {
   if (!p || !buf) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_serialize: null");
+  HB_TRY(check_dense(p, "hb_poly_serialize"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_poly_serialize", true));
   uint64_t need; hb_poly_serialized_size(p, n, &need);
@@ -525,6 +558,7 @@ extern "C" int hb_poly_serialize(hb_poly* p, const int32_t* idx, int n, void* bu
 // idx_out receives the index set (capacity nprimes), *n_out its size; rows are uploaded into p.
 extern "C" int hb_poly_deserialize(hb_poly* p, const void* buf, uint64_t buflen, int32_t* idx_out, int* n_out) {
   if (!p || !buf || !idx_out || !n_out) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_deserialize: null");
+  HB_TRY(check_dense(p, "hb_poly_deserialize"));
   hb_ctx* c = p->ctx;
   const unsigned char* o = (const unsigned char*)buf; const unsigned char* end = o + buflen;
   if (buflen < 8) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_deserialize: truncated");
@@ -568,59 +602,195 @@ static int prg_grow(hb_ctx* c, void** p, size_t* cap, size_t bytes) {
   *cap = bytes;
   return HB_OK;
 }
-extern "C" int hb_poly_randomize(hb_poly* const* polys, int npolys, const int32_t* idx, int n, const uint8_t* seed, int seedlen) {
-  static const char* who = "hb_poly_randomize";
-  if (!polys || npolys <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: no polynomials", who);
-  if (seedlen < 0 || (seedlen > 0 && !seed)) return hb_fail(HB_ERR_BAD_ARG, "%s: null seed with length %d", who, seedlen);
-  hb_ctx* c = nullptr;
-  HB_TRY(check_polys(polys, npolys, &c, who));
-  HB_TRY(check_idx(c, idx, n, who, true));
-  for (int i = 1; i < n; i++) if (idx[i] <= idx[i - 1]) return hb_fail(HB_ERR_BAD_ARG, "%s: prime indices must be strictly ascending", who);
-  if (n == 0) return HB_OK;
-  const HbPrgKey key = hb_prg_derive_key(seed, seedlen);
-  const u64 N = c->N;
-  const int T = npolys * n;
-  std::vector<HbPrgRow> rows((size_t)T);
-  int wmax = 1;
+// candidate format and counting window of schedule row p*n + r (prime idx[r]); row pointers unset
+static void prg_rows(hb_ctx* c, int npolys, const int32_t* idx, int n, std::vector<HbPrgRow>& rows, int* wmax) {
+  rows.assign((size_t)npolys * n, HbPrgRow{});
+  *wmax = 1;
   for (int r = 0; r < n; r++) {
     const u64 q = c->q[idx[r]];
     const int k = h_bitlen(q - 1), nb = (k + 7) / 8;
-    const int w = c->prg_window ? c->prg_window : hb_prg_window(q, k, nb, N);
-    wmax = std::max(wmax, w);
+    const int w = c->prg_window ? c->prg_window : hb_prg_window(q, k, nb, c->N);
+    *wmax = std::max(*wmax, w);
     for (int p = 0; p < npolys; p++) {
       HbPrgRow& R = rows[(size_t)p * n + r];
-      R.q = q; R.mask = k >= 64 ? ~0ULL : (1ULL << k) - 1; R.nb = nb; R.window = w;
-      R.row = polys[p]->d + (size_t)idx[r] * N;
+      R.q = q; R.mask = k >= 64 ? ~0ULL : (1ULL << k) - 1; R.nb = nb; R.window = w; R.row = nullptr;
     }
   }
-  HB_TRY(prg_grow(c, (void**)&c->prg_start, &c->prg_start_cap, (size_t)(T + 1) * sizeof(u64)));
-  HB_TRY(prg_grow(c, (void**)&c->prg_off, &c->prg_off_cap, (size_t)T * wmax * sizeof(unsigned)));
+}
+// Step (a), the schedule: the chain of k_prg_count launches over rows[0..T).  start[0] = 0 (a fresh SetSeed); each launch
+// reads its row's first buffer from device memory, writes the next row's and its buffers' row offsets at off + t*wstride.
+static int prg_count_chain(hb_ctx* c, const HbPrgKey& key, const HbPrgRow* rows, int T, u64* start, unsigned* off, int wstride) {
   if (!c->prg_ticket) {
     HB_TRY(ctx_alloc(c, (void**)&c->prg_ticket, sizeof(unsigned long long)));
     HB_CUDA(cudaMemsetAsync(c->prg_ticket, 0, sizeof(unsigned long long), c->stream));
   }
-  HB_CUDA(cudaMemsetAsync(c->prg_start, 0, sizeof(u64), c->stream));   // a fresh SetSeed: the first row starts at buffer 0
-  // the row chain: each launch reads its row's first buffer from device memory and writes the next row's
+  HB_CUDA(cudaMemsetAsync(start, 0, sizeof(u64), c->stream));
   HbPrgCountJob C;
-  C.key = key; C.N = N; C.start = c->prg_start; C.ticket = c->prg_ticket;
+  C.key = key; C.N = c->N; C.start = start; C.ticket = c->prg_ticket;
   for (int t = 0; t < T; t++) {
-    C.r = rows[(size_t)t]; C.t = t; C.off = c->prg_off + (size_t)t * wmax;
+    C.r = rows[t]; C.t = t; C.off = off + (size_t)t * wstride;
     pre_launch(c);
     HB_LAUNCH(k_prg_count, dim3((unsigned)((C.r.window + HB_PRG_WARPS - 1) / HB_PRG_WARPS)), dim3(HB_PRG_THREADS), HB_PRG_SMEM_BYTES, c->stream, C);
     HB_TRY(post_launch(c, "k_prg_count", (u64)C.r.window * sizeof(unsigned) * 2));
   }
-  // every (row, buffer) at once
+  return HB_OK;
+}
+// Step (b), the values: rows[i] (row pointer set) from schedule row sr[i], up to HB_PRG_MAXT rows per k_prg_fill launch
+static int prg_fill(hb_ctx* c, const HbPrgKey& key, const u64* start, const unsigned* off, int wstride, const HbPrgRow* rows, const unsigned* sr, int T) {
   HbPrgFillJob F;
-  F.key = key; F.N = N; F.start = c->prg_start; F.off = c->prg_off; F.wmax = wmax;
+  F.key = key; F.N = c->N; F.start = start; F.off = off; F.wstride = wstride;
   for (int t0 = 0; t0 < T; t0 += HB_PRG_MAXT) {
     const int nt = std::min(HB_PRG_MAXT, T - t0);
-    F.t0 = t0;
-    for (int i = 0; i < nt; i++) F.r[i] = rows[(size_t)t0 + i];
+    int wl = 1;
+    for (int i = 0; i < nt; i++) { F.r[i] = rows[t0 + i]; F.sr[i] = sr[t0 + i]; wl = std::max(wl, F.r[i].window); }
     pre_launch(c);
-    HB_LAUNCH(k_prg_fill, dim3((unsigned)((wmax + HB_PRG_WARPS - 1) / HB_PRG_WARPS), (unsigned)nt), dim3(HB_PRG_THREADS), HB_PRG_SMEM_BYTES, c->stream, F);
-    HB_TRY(post_launch(c, "k_prg_fill", (u64)nt * N * 8));
+    HB_LAUNCH(k_prg_fill, dim3((unsigned)((wl + HB_PRG_WARPS - 1) / HB_PRG_WARPS), (unsigned)nt), dim3(HB_PRG_THREADS), HB_PRG_SMEM_BYTES, c->stream, F);
+    HB_TRY(post_launch(c, "k_prg_fill", (u64)nt * c->N * 8));
   }
   return HB_OK;
+}
+static int prg_args(hb_ctx* c, const int32_t* idx, int n, const uint8_t* seed, int seedlen, const char* who) {
+  if (seedlen < 0 || (seedlen > 0 && !seed)) return hb_fail(HB_ERR_BAD_ARG, "%s: null seed with length %d", who, seedlen);
+  HB_TRY(check_idx(c, idx, n, who, true));
+  for (int i = 1; i < n; i++) if (idx[i] <= idx[i - 1]) return hb_fail(HB_ERR_BAD_ARG, "%s: prime indices must be strictly ascending", who);
+  return HB_OK;
+}
+extern "C" int hb_poly_randomize(hb_poly* const* polys, int npolys, const int32_t* idx, int n, const uint8_t* seed, int seedlen) {
+  static const char* who = "hb_poly_randomize";
+  if (!polys || npolys <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: no polynomials", who);
+  hb_ctx* c = nullptr;
+  HB_TRY(check_polys(polys, npolys, &c, who));
+  HB_TRY(prg_args(c, idx, n, seed, seedlen, who));
+  if (n == 0) return HB_OK;
+  const HbPrgKey key = hb_prg_derive_key(seed, seedlen);
+  const int T = npolys * n;
+  std::vector<HbPrgRow> rows;
+  int wmax;
+  prg_rows(c, npolys, idx, n, rows, &wmax);
+  std::vector<unsigned> sr((size_t)T);
+  for (int p = 0; p < npolys; p++)
+    for (int r = 0; r < n; r++) { rows[(size_t)p * n + r].row = polys[p]->d + (size_t)idx[r] * c->N; sr[(size_t)p * n + r] = (unsigned)(p * n + r); }
+  // the schedule lives in context scratch for this call only; every row is filled
+  HB_TRY(prg_grow(c, (void**)&c->prg_start, &c->prg_start_cap, (size_t)(T + 1) * sizeof(u64)));
+  HB_TRY(prg_grow(c, (void**)&c->prg_off, &c->prg_off_cap, (size_t)T * wmax * sizeof(unsigned)));
+  HB_TRY(prg_count_chain(c, key, rows.data(), T, c->prg_start, c->prg_off, wmax));
+  return prg_fill(c, key, c->prg_start, c->prg_off, wmax, rows.data(), sr.data(), T);
+}
+
+// The schedule's device storage for stride wmax: start[T+1], then off[T*wmax]
+static int sched_alloc(hb_ctx* c, HbSeedSched* S) {
+  const size_t T = S->rows.size();
+  if (S->blk) { HB_CUDA(cudaFree(S->blk)); c->bytes -= S->bytes; S->blk = nullptr; }
+  S->bytes = (T + 1) * sizeof(u64) + T * (size_t)S->wmax * sizeof(unsigned);
+  HB_TRY(ctx_alloc(c, &S->blk, S->bytes));
+  S->start = (u64*)S->blk;
+  S->off = (unsigned*)(S->start + T + 1);
+  return HB_OK;
+}
+static int sched_build(hb_ctx* c, HbSeedSched* S) {
+  const int T = (int)S->rows.size();
+  if (T == 0) return HB_OK;
+  HB_TRY(sched_alloc(c, S));
+  HB_TRY(prg_count_chain(c, S->key, S->rows.data(), T, S->start, S->off, S->wmax));
+  // k_prg_count finishes a row that needs more buffers than its window on its slow path and records no offsets for the extra
+  // buffers.  Each row's need is start[t+1] - start[t]: rows that outgrew their window are counted again with exactly that
+  // window (the starts do not change), so every buffer of every row has its offset.
+  std::vector<u64> st((size_t)T + 1);
+  HB_CUDA(cudaMemcpyAsync(st.data(), S->start, st.size() * sizeof(u64), cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  bool short_rows = false;
+  for (int t = 0; t < T; t++) {
+    const int need = (int)(st[(size_t)t + 1] - st[(size_t)t]);
+    if (need > S->rows[(size_t)t].window) { S->rows[(size_t)t].window = need; S->wmax = std::max(S->wmax, need); short_rows = true; }
+  }
+  if (!short_rows) return HB_OK;
+  HB_TRY(sched_alloc(c, S));
+  return prg_count_chain(c, S->key, S->rows.data(), T, S->start, S->off, S->wmax);
+}
+extern "C" int hb_poly_create_seeded(hb_ctx* c, int npolys, const int32_t* idx, int n, const uint8_t* seed, int seedlen, hb_poly** out) {
+  static const char* who = "hb_poly_create_seeded";
+  if (!c || !out) return hb_fail(HB_ERR_BAD_ARG, "%s: null", who);
+  if (npolys <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: no polynomials", who);
+  HB_TRY(prg_args(c, idx, n, seed, seedlen, who));
+  HbSeedSched* S = new HbSeedSched();
+  S->key = hb_prg_derive_key(seed, seedlen);
+  S->idx.assign(idx, idx + n);
+  prg_rows(c, npolys, idx, n, S->rows, &S->wmax);
+  const int rc = sched_build(c, S);
+  if (rc != HB_OK) {
+    cudaStreamSynchronize(c->stream);
+    if (S->blk) { cudaFree(S->blk); c->bytes -= S->bytes; }
+    delete S;
+    return rc;
+  }
+  for (int p = 0; p < npolys; p++) {
+    hb_poly* h = new hb_poly();
+    h->ctx = c; h->d = nullptr; h->owned = false; h->sched = S; h->sched_poly = p;
+    out[p] = h;
+  }
+  S->refs = npolys;
+  return HB_OK;
+}
+// rows idx of seeded[p] into the rows of dst[p]: every row is checked against its set before anything is launched, then one
+// k_prg_fill launch per schedule (one in practice: the a_i of a matrix share a seed)
+static int prg_expand(hb_ctx* c, hb_poly* const* seeded, u64* const* dst, int np, const int32_t* idx, int n, const char* who) {
+  std::vector<unsigned> srow((size_t)np * n);
+  for (int p = 0; p < np; p++) {
+    const HbSeedSched* S = seeded[p]->sched;
+    const int ns = (int)S->idx.size();
+    for (int r = 0; r < n; r++) {
+      const auto it = std::lower_bound(S->idx.begin(), S->idx.end(), idx[r]);
+      if (it == S->idx.end() || *it != idx[r]) return hb_fail(HB_ERR_INDEX_SET, "%s: row %d is not in the seeded set", who, idx[r]);
+      srow[(size_t)p * n + r] = (unsigned)(seeded[p]->sched_poly * ns + (int)(it - S->idx.begin()));
+    }
+  }
+  std::vector<char> done((size_t)np, 0);
+  for (int p0 = 0; p0 < np; p0++) {
+    if (done[(size_t)p0]) continue;
+    const HbSeedSched* S = seeded[p0]->sched;
+    std::vector<HbPrgRow> rows; std::vector<unsigned> sr;
+    for (int p = p0; p < np; p++) {
+      if (seeded[p]->sched != S) continue;
+      done[(size_t)p] = 1;
+      for (int r = 0; r < n; r++) {
+        const unsigned s = srow[(size_t)p * n + r];
+        HbPrgRow R = S->rows[s];
+        R.row = dst[p] + (size_t)idx[r] * c->N;
+        rows.push_back(R); sr.push_back(s);
+      }
+    }
+    HB_TRY(prg_fill(c, S->key, S->start, S->off, S->wmax, rows.data(), sr.data(), (int)rows.size()));
+  }
+  return HB_OK;
+}
+extern "C" int hb_poly_expand(hb_poly* const* seeded, hb_poly* const* dst, int npolys, const int32_t* idx, int n) {
+  static const char* who = "hb_poly_expand";
+  if (!seeded || npolys <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: no polynomials", who);
+  hb_ctx* c = nullptr;
+  HB_TRY(check_polys(seeded, npolys, &c, who, true));
+  for (int p = 0; p < npolys; p++) if (!seeded[p]->sched) return hb_fail(HB_ERR_BAD_ARG, "%s: seeded[%d] is not a seeded polynomial", who, p);
+  HB_TRY(check_polys(dst, npolys, &c, who));
+  HB_TRY(check_idx(c, idx, n, who, true));
+  if (n == 0) return HB_OK;
+  std::vector<u64*> d((size_t)npolys);
+  for (int p = 0; p < npolys; p++) d[(size_t)p] = dst[p]->d;
+  return prg_expand(c, seeded, d.data(), npolys, idx, n, who);
+}
+// The seeded entries of evk_a[0..nd): rows idx of each are regenerated into the context's key scratch (nd full-height polys,
+// apart from the digit pool; allocated on first use, so a later call neither allocates nor synchronises and stays capturable
+// in a CUDA graph).  `use` receives evk_a with those entries replaced.  The entry points call this once per call, before
+// their item chunks.
+static int ks_expand_a(hb_ctx* c, hb_poly* const* evk_a, int nd, const int32_t* idx, int n, std::vector<hb_poly*>& use) {
+  use.assign(evk_a, evk_a + nd);
+  std::vector<hb_poly*> src; std::vector<u64*> dst;
+  for (int i = 0; i < nd; i++) {
+    if (!evk_a[i]->sched) continue;
+    while ((int)c->ks_a.size() <= i) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->ks_a.push_back(p); }
+    use[(size_t)i] = c->ks_a[(size_t)i];
+    src.push_back(evk_a[i]); dst.push_back(c->ks_a[(size_t)i]->d);
+  }
+  if (src.empty()) return HB_OK;
+  return prg_expand(c, src.data(), dst.data(), (int)src.size(), idx, n, "key switch (evk_a)");
 }
 
 static int pool_get(hb_ctx* c, int n, std::vector<hb_poly*>& out) {
@@ -1479,6 +1649,7 @@ extern "C" int hb_scale_down_norm(hb_poly* const* polys, int nitems, const int32
 }
 extern "C" int hb_to_poly(hb_poly* p, const int32_t* idx, int n, int positive, uint64_t* out, int Lout) {
   if (!p || !out) return hb_fail(HB_ERR_BAD_ARG, "hb_to_poly: null");
+  HB_TRY(check_dense(p, "hb_to_poly"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_to_poly", true));
   if (n == 0) { memset(out, 0, sizeof(u64) * c->N * Lout); return HB_OK; }  // src/DoubleCRT.cpp:931-935
@@ -1509,6 +1680,7 @@ extern "C" int hb_to_poly(hb_poly* p, const int32_t* idx, int n, int positive, u
 
 extern "C" int hb_to_poly_mod_p(hb_poly* p, const int32_t* idx, int n, uint64_t ptxt_space, uint64_t factor, int64_t* out) {
   if (!p || !out) return hb_fail(HB_ERR_BAD_ARG, "hb_to_poly_mod_p: null");
+  HB_TRY(check_dense(p, "hb_to_poly_mod_p"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_to_poly_mod_p", true));
   if (ptxt_space < 2) return hb_fail(HB_ERR_BAD_ARG, "hb_to_poly_mod_p: ptxt_space must be >= 2");
@@ -1684,6 +1856,7 @@ static int to_powerful_rows(hb_ctx* c, hb_poly* p, const int32_t* idx, int n, co
 }
 extern "C" int hb_dcrt_to_powerful(hb_poly* p, const int32_t* idx, int n, uint64_t* out, int Lout) {
   if (!p || !out) return hb_fail(HB_ERR_BAD_ARG, "hb_dcrt_to_powerful: null");
+  HB_TRY(check_dense(p, "hb_dcrt_to_powerful"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_dcrt_to_powerful"));
   if (Lout < n) return hb_fail(HB_ERR_BAD_ARG, "hb_dcrt_to_powerful: Lout=%d limbs cannot hold a %d-prime product", Lout, n);
@@ -1703,6 +1876,7 @@ extern "C" int hb_dcrt_to_powerful(hb_poly* p, const int32_t* idx, int n, uint64
 }
 extern "C" int hb_raw_mod_switch(hb_poly* p, const int32_t* idx, int n, uint64_t q, uint64_t p2r, int64_t* out) {
   if (!p || !out) return hb_fail(HB_ERR_BAD_ARG, "hb_raw_mod_switch: null");
+  HB_TRY(check_dense(p, "hb_raw_mod_switch"));
   hb_ctx* c = p->ctx;
   HB_TRY(check_idx(c, idx, n, "hb_raw_mod_switch"));
   if (q <= 1) return hb_fail(HB_ERR_BAD_ARG, "q must be greater than 1");                                  // src/Ctxt.cpp:2953
@@ -1764,6 +1938,7 @@ extern "C" int hb_conv_make_y_bcast(hb_poly* const* polys, int nitems, const int
   HB_TRY(check_idx(c, D, nD, "hb_conv_make_y_bcast")); HB_TRY(check_idx(c, owned, nOwned, "hb_conv_make_y_bcast(owned)", true));
   if (c->gen.on) return hb_fail(HB_ERR_UNSUPPORTED, "prime-sharded conversion is only built for power-of-two m");
   if (npeers < 0 || npeers > HB_MAXPEERS || (npeers && !peer_ypolys)) return hb_fail(HB_ERR_BAD_ARG, "hb_conv_make_y_bcast: npeers out of range");
+  for (int i = 0; i < npeers * nitems; i++) if (peer_ypolys[i]) HB_TRY(check_dense(peer_ypolys[i], "hb_conv_make_y_bcast(peers)"));
   if (nOwned == 0) return HB_OK;
   if (nOwned > HB_MAXROWS) return hb_fail(HB_ERR_UNSUPPORTED, "hb_conv_make_y_bcast: more than %d owned rows", HB_MAXROWS);
   std::vector<u64> sc(nOwned);
@@ -1803,6 +1978,7 @@ extern "C" int hb_conv_make_y_bcast(hb_poly* const* polys, int nitems, const int
 // CUDA IPC: export a polynomial's device buffer / map a peer's buffer (one process per GPU)
 extern "C" int hb_poly_ipc_export(hb_poly* p, void* handle64) {
   if (!p || !handle64) return hb_fail(HB_ERR_BAD_ARG, "hb_poly_ipc_export: null");
+  HB_TRY(check_dense(p, "hb_poly_ipc_export"));
 #ifdef HB_SIM
   return hb_fail(HB_ERR_UNSUPPORTED, "CUDA IPC is not available in the simulator");
 #else
@@ -1945,6 +2121,9 @@ extern "C" int hb_automorph_keyswitch_digits(hb_poly* const* digits, int maxdig,
   if (ndig <= 0 || ndig > maxdig) return hb_fail(HB_ERR_BAD_ARG, "hb_automorph_keyswitch_digits: ndig=%d out of range", ndig);
   for (int i = 0; i < nitems; i++) if (c0[i] == out0[i] || c0[i] == out1[i]) return hb_fail(HB_ERR_BAD_ARG, "hb_automorph_keyswitch_digits: outputs must not alias c0");
   for (int i = 0; i < nitems * maxdig; i++) for (int j = 0; j < nitems; j++) if (digits[i] == out0[j] || digits[i] == out1[j]) return hb_fail(HB_ERR_BAD_ARG, "hb_automorph_keyswitch_digits: outputs must not alias the digits");
+  HB_TRY(check_polys(out0, nitems, &c, "hb_automorph_keyswitch_digits(out0)")); HB_TRY(check_polys(out1, nitems, &c, "hb_automorph_keyswitch_digits(out1)"));
+  HB_TRY(check_polys(digits, nitems * maxdig, &c, "hb_automorph_keyswitch_digits(digits)"));
+  HB_TRY(check_polys(evk_a, ndig, &c, "hb_automorph_keyswitch_digits(evk_a)", true)); HB_TRY(check_polys(evk_b, ndig, &c, "hb_automorph_keyswitch_digits(evk_b)"));
   std::vector<int32_t> Sp(S, S + nS); Sp.insert(Sp.end(), c->special.begin(), c->special.end()); std::sort(Sp.begin(), Sp.end());
   std::vector<u64> sc(Sp.size(), 0);
   for (size_t r = 0; r < Sp.size(); r++)
@@ -1975,9 +2154,11 @@ static int keyswitch_digits_impl(hb_poly* const* digits, int maxdig, int ndig, i
   hb_ctx* c = nullptr;
   HB_TRY(check_polys(out0, nitems, &c, "hb_keyswitch_digits")); HB_TRY(check_polys(out1, nitems, &c, "hb_keyswitch_digits"));
   if (ndig <= 0 || ndig > HB_MAXDIG || ndig > maxdig) return hb_fail(HB_ERR_BAD_ARG, "hb_keyswitch_digits: ndig=%d out of range", ndig);
-  HB_TRY(check_polys(evk_a, ndig, &c, "hb_keyswitch_digits(evk_a)")); HB_TRY(check_polys(evk_b, ndig, &c, "hb_keyswitch_digits(evk_b)"));
+  HB_TRY(check_polys(evk_a, ndig, &c, "hb_keyswitch_digits(evk_a)", true)); HB_TRY(check_polys(evk_b, ndig, &c, "hb_keyswitch_digits(evk_b)"));
   HB_TRY(check_polys(digits, nitems * maxdig, &c, "hb_keyswitch_digits(digits)"));
   HB_TRY(check_idx(c, idx, n, "hb_keyswitch_digits"));
+  // a seeded evk_a is regenerated here, before the item chunks; the fused relinearisation hands in entries it already regenerated
+  std::vector<hb_poly*> ka; HB_TRY(ks_expand_a(c, evk_a, ndig, idx, n, ka)); evk_a = ka.data();
   return for_items(nitems, [&](int i0, int nit) {
     for (int r0 = 0; r0 < n; r0 += HB_MAXROWS) {
       int nr = std::min(HB_MAXROWS, n - r0);
@@ -2135,6 +2316,18 @@ static int relin_fused_v1(hb_ctx* c, hb_poly* const* c0, hb_poly* const* c1, hb_
   });
 }
 
+// The checks of the key and the regeneration of a seeded evk_a for a relinearisation over S: the matrix must have a column
+// for every digit of S (src/DoubleCRT.cpp:485-493), and only those columns are read.
+static int relin_key(hb_ctx* c, const int32_t* S, int nS, const std::vector<int32_t>& Sp, hb_poly* const* evk_a, hb_poly* const* evk_b,
+                     int ndig_evk, const char* who, std::vector<hb_poly*>& ka) {
+  for (int i = 0; i < nS; i++) if (c->digit_of[S[i]] < 0) return hb_fail(HB_ERR_INDEX_SET, "breakIntoDigits: index set must be a subset of ctxt primes (prime %d)", S[i]);
+  std::vector<char> rem(c->nprimes, 0); int left = nS, nd = 0;
+  for (int i = 0; i < nS; i++) rem[S[i]] = 1;
+  for (; left > 0; nd++) for (int i = 0; i < c->nprimes; i++) if (rem[i] && c->digit_of[i] == nd) { rem[i] = 0; left--; }
+  if (nd > ndig_evk) return hb_fail(HB_ERR_BAD_ARG, "%s: key-switching matrix has %d columns, need %d", who, ndig_evk, nd);
+  hb_ctx* cx = c; HB_TRY(check_polys(evk_a, nd, &cx, who, true)); HB_TRY(check_polys(evk_b, nd, &cx, who));
+  return ks_expand_a(c, evk_a, nd, Sp.data(), (int)Sp.size(), ka);
+}
 extern "C" int hb_relinearize(hb_poly* const* c0, hb_poly* const* c1, hb_poly* const* c2, int nitems,
                               const int32_t* S, int nS, hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk) {
   hb_ctx* c = nullptr;
@@ -2144,6 +2337,8 @@ extern "C" int hb_relinearize(hb_poly* const* c0, hb_poly* const* c1, hb_poly* c
   const int maxdig = c->ndigits;
   std::vector<hb_poly*> dig; HB_TRY(pool_get(c, nitems * maxdig, dig));
   std::vector<int32_t> Sp(S, S + nS); Sp.insert(Sp.end(), c->special.begin(), c->special.end()); std::sort(Sp.begin(), Sp.end());
+  // a seeded key: its a_i are regenerated once for the whole call, on the rows S | special, before either path below
+  std::vector<hb_poly*> ka; HB_TRY(relin_key(c, S, nS, Sp, evk_a, evk_b, ndig_evk, "hb_relinearize", ka)); evk_a = ka.data();
   // a digit below the last live one may have no live prime (an index set with a hole): the reference then carries a zero digit
   // and still divides the later ones by that digit's full product (src/DoubleCRT.cpp:488-493,509-561); the fused path converts
   // from the digit's own rows and has nothing to convert from, so such sets take the step-by-step path below
@@ -2178,6 +2373,9 @@ extern "C" int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_p
   for (int i = 0; i < nS; i++)
     if (std::find(S_in, S_in + nS_in, S[i]) == S_in + nS_in)
       return hb_fail(HB_ERR_INDEX_SET, "hb_mul_relin_moddown: the common set must be a subset of the operands' set (prime %d)", S[i]);
+  HB_TRY(check_idx(c, S, nS, "hb_mul_relin_moddown"));
+  std::vector<int32_t> Sp(S, S + nS); Sp.insert(Sp.end(), c->special.begin(), c->special.end()); std::sort(Sp.begin(), Sp.end());
+  std::vector<hb_poly*> ka; HB_TRY(relin_key(c, S, nS, Sp, evk_a, evk_b, ndig_evk, "hb_mul_relin_moddown", ka)); evk_a = ka.data();
   std::vector<hb_poly*> allp;
   for (int i = 0; i < nitems; i++) { allp.push_back(a0[i]); allp.push_back(a1[i]); allp.push_back(b0[i]); allp.push_back(b1[i]); }
   HB_TRY(scale_down_impl(allp.data(), (int)allp.size(), S_in, nS_in, S, nS, ptxt_space, nullptr, c->gen.on ? 0 : 1));   // lazy rows: the tensor product reduces exactly
@@ -2186,7 +2384,6 @@ extern "C" int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_p
   // reLinearize (src/Ctxt.cpp:720-786)
   HB_TRY(hb_relinearize(a0, a1, b0, nitems, S, nS, evk_a, evk_b, ndig_evk));
   // drop the special primes again: modDownToSet(ctxtPrimes) (src/Ctxt.cpp:589-593)
-  std::vector<int32_t> Sp(S, S + nS); Sp.insert(Sp.end(), c->special.begin(), c->special.end()); std::sort(Sp.begin(), Sp.end());
   std::vector<hb_poly*> two;
   for (int i = 0; i < nitems; i++) { two.push_back(a0[i]); two.push_back(a1[i]); }
   return hb_scale_down(two.data(), (int)two.size(), Sp.data(), (int)Sp.size(), S, nS, ptxt_space);

@@ -358,6 +358,31 @@ class Engine:
         buf = (C.c_uint8 * max(1, len(seed))).from_buffer_copy(seed or b"\0")
         self._ck(self.lib.hb_poly_randomize(_arr(polys), len(polys), p, n, buf, len(seed)))
 
+    def seeded(self, npolys, idx, seed):
+        """The rows randomize(npolys polys, idx, seed) would write, kept as the seed plus a row schedule
+        (hb_poly_create_seeded).  The returned Polys have no rows: they go in any evk_a list, where the key switch
+        regenerates the rows it reads, and to expand()."""
+        if isinstance(seed, int):
+            if seed < 0:
+                raise ValueError("seed must be non-negative")
+            seed = seed.to_bytes((seed.bit_length() + 7) // 8, "little")
+        seed = bytes(seed)
+        a, p, n = _idx(idx)
+        buf = (C.c_uint8 * max(1, len(seed))).from_buffer_copy(seed or b"\0")
+        hs = (C.c_void_p * max(1, npolys))()
+        self._ck(self.lib.hb_poly_create_seeded(self.h, int(npolys), p, n, buf, len(seed), hs))
+        out = []
+        for h in hs[:npolys]:
+            q = Poly.__new__(Poly)
+            q.eng, q.h = self, C.c_void_p(h)
+            out.append(q)
+        return out
+
+    def expand(self, seeded, dst, idx):
+        """Rows idx of each seeded Poly into the ordinary Poly beside it in dst (hb_poly_expand)."""
+        a, p, n = _idx(idx)
+        self._ck(self.lib.hb_poly_expand(_arr(seeded), _arr(dst), len(seeded), p, n))
+
 
 class Chain:
     """Host-side prime chain (hb_chain): helib::Context::buildModChain reproduced in C++."""
