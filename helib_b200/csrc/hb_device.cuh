@@ -727,6 +727,85 @@ __global__ void __launch_bounds__(HB_THREADS) k_ks_inner(const HbPrimeDev* __res
   }
 }
 
+// Hoisted linear map (the loop body of MatMul1DExec::mul's native FULL branch, src/matmul.cpp:1226-1252): for every amount t
+// of the launch, the hoisted key switch of k_ks_inner mode 2 times the constant cst[t], summed over the amounts:
+//   acc0 (+)= sum_t cst_t * ( scal*sigma_kt(c0) + [k_t != 1] sum_i sigma_kt(D_i)*b_{t,i} )
+//   acc1 (+)= sum_t cst_t * ( [k_t == 1] scal*c1 + [k_t != 1] sum_i sigma_kt(D_i)*a_{t,i} )
+// Each inner product is summed in 128 bits and reduced once; its products with the constants are summed in 128 bits across
+// the amounts and reduced once, when the accumulators are written.  All terms are below 2^120 (q < 2^60), so 255 fit:
+// at most HB_LINMAP_MAXAMT amounts plus the accumulator's old value.
+#define HB_LINMAP_MAXAMT 64
+struct HbLinJob {
+  u64 N, m;
+  const int* rep; const int* irep;   // general m: sigma_k(x)[j] = x[irep[rep[j]*k mod m]];  null: power-of-two m
+  int ndig, nitems, namt, accumulate;
+  HbRows rows;
+  u64 scal[HB_MAXROWS];              // P mod q on the rows of S, 0 on the special rows (addPrimesAndScale)
+  u64 k[HB_LINMAP_MAXAMT];
+  const u64* cst[HB_LINMAP_MAXAMT];
+  const u64* evk_a[HB_LINMAP_MAXAMT][HB_MAXDIG];
+  const u64* evk_b[HB_LINMAP_MAXAMT][HB_MAXDIG];
+  const u64* dig[HB_MAXB][HB_MAXDIG];
+  const u64* c0[HB_MAXB];
+  const u64* c1[HB_MAXB];
+  u64* acc0[HB_MAXB];
+  u64* acc1[HB_MAXB];
+};
+// grid = (coefficient blocks, rows, item groups of NI): the NI items of a group share every key and constant word a thread
+// loads, and keep their accumulators in registers (NI is a template parameter, so the per-item arrays are fully unrolled).
+template <int NI>
+__global__ void __launch_bounds__(HB_THREADS) k_ks_linmap(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT HbLinJob J) {
+  const int pi = J.rows.prime[blockIdx.y];
+  const HbPrimeDev P = primes[pi];
+  const size_t N = (size_t)J.N;
+  const size_t off = (size_t)pi * N;
+  const u64 sc = J.scal[blockIdx.y];
+  const int it0 = blockIdx.z * NI;
+  const int cnt = J.nitems - it0 < NI ? J.nitems - it0 : NI;
+  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < N; j += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = off + j;
+    u64 h0[NI], l0[NI], h1[NI], l1[NI];
+#pragma unroll
+    for (int u = 0; u < NI; u++) {
+      h0[u] = 0; l0[u] = 0; h1[u] = 0; l1[u] = 0;
+      if (J.accumulate && u < cnt) { l0[u] = J.acc0[it0 + u][o]; l1[u] = J.acc1[it0 + u][o]; }
+    }
+    const u64 rj = J.rep ? (u64)J.rep[j] : 2 * (u64)j + 1;   // m <= 2^20: rj*k < 2^41
+    for (int t = 0; t < J.namt; t++) {
+      const u64 k = J.k[t];
+      const u64 cw = J.cst[t][o];
+      if (k == 1) {   // no automorphism, no key switch: cst * P * (c0, c1)
+        const u64 scw = hb_mulmod(sc, cw, P);
+#pragma unroll
+        for (int u = 0; u < NI; u++)
+          if (u < cnt) { hb_mac128(h0[u], l0[u], J.c0[it0 + u][o], scw); hb_mac128(h1[u], l1[u], J.c1[it0 + u][o], scw); }
+        continue;
+      }
+      const size_t g = off + (J.rep ? (size_t)J.irep[(rj * k) % J.m] : (size_t)(((rj * k) & (J.m - 1)) >> 1));
+      u64 p0h[NI], p0l[NI], p1h[NI], p1l[NI];
+#pragma unroll
+      for (int u = 0; u < NI; u++) {
+        p0h[u] = 0; p0l[u] = 0; p1h[u] = 0; p1l[u] = 0;
+        if (sc && u < cnt) hb_mac128(p0h[u], p0l[u], J.c0[it0 + u][g], sc);
+      }
+      for (int i = 0; i < J.ndig; i++) {
+        const u64 b = J.evk_b[t][i][o], a = J.evk_a[t][i][o];
+#pragma unroll
+        for (int u = 0; u < NI; u++)
+          if (u < cnt) { const u64 d = J.dig[it0 + u][i][g]; hb_mac128(p0h[u], p0l[u], d, b); hb_mac128(p1h[u], p1l[u], d, a); }
+      }
+#pragma unroll
+      for (int u = 0; u < NI; u++) {
+        hb_mac128(h0[u], l0[u], hb_reduce128(p0h[u], p0l[u], P), cw);
+        hb_mac128(h1[u], l1[u], hb_reduce128(p1h[u], p1l[u], P), cw);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < NI; u++)
+      if (u < cnt) { J.acc0[it0 + u][o] = hb_reduce128(h0[u], l0[u], P); J.acc1[it0 + u][o] = hb_reduce128(h1[u], l1[u], P); }
+  }
+}
+
 
 // ------------------------------------------------------------------------------------------
 // Canonical-embedding norm (noise metadata): max_j |f(zeta^(2j+1))|, zeta = e^(i*pi/N), in FP64.

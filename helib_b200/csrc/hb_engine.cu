@@ -16,6 +16,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -779,7 +780,9 @@ extern "C" int hb_poly_expand(hb_poly* const* seeded, hb_poly* const* dst, int n
 // The seeded entries of evk_a[0..nd): rows idx of each are regenerated into the context's key scratch (nd full-height polys,
 // apart from the digit pool; allocated on first use, so a later call neither allocates nor synchronises and stays capturable
 // in a CUDA graph).  `use` receives evk_a with those entries replaced.  The entry points call this once per call, before
-// their item chunks.
+// their item chunks.  hb_hoisted_linear_map calls it once per group of amounts, with at most HB_LINMAP_SEEDED entries
+// (whole matrices), so the scratch holds at most max(HB_MAXDIG, HB_LINMAP_SEEDED) polys whatever the number of amounts.
+#define HB_LINMAP_SEEDED (2 * HB_MAXDIG)
 static int ks_expand_a(hb_ctx* c, hb_poly* const* evk_a, int nd, const int32_t* idx, int n, std::vector<hb_poly*>& use) {
   use.assign(evk_a, evk_a + nd);
   std::vector<hb_poly*> src; std::vector<u64*> dst;
@@ -2199,6 +2202,111 @@ static int keyswitch_digits_impl(hb_poly* const* digits, int maxdig, int ndig, i
     }
     return HB_OK;
   });
+}
+
+// Hoisted linear map (SURVEY 8f-1): the loop body of MatMul1DExec::mul's native FULL branch (src/matmul.cpp:1226-1252),
+// sum_j consts[j] * BasicAutomorphPrecon::automorph(k[j]), in one k_ks_linmap launch per group of up to HB_LINMAP_MAXAMT
+// amounts (and per item chunk and row chunk).  No permuted digit copies and no intermediate rows: sigma_k is applied while
+// the digits and c0 are loaded, for general m too.
+extern "C" int hb_hoisted_linear_map(hb_poly* const* digits, int maxdig, int ndig, int nitems, const int32_t* S, int nS,
+                                     hb_poly* const* c0, hb_poly* const* c1, int namt, const uint64_t* k, hb_poly* const* consts,
+                                     hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* acc0, hb_poly* const* acc1,
+                                     int accumulate) {
+  static const char* who = "hb_hoisted_linear_map";
+  hb_ctx* c = nullptr;
+  HB_TRY(check_polys(c0, nitems, &c, who));
+  HB_TRY(check_idx(c, S, nS, who));
+  if (namt <= 0 || !k || !consts) return hb_fail(HB_ERR_BAD_ARG, "%s: no amounts", who);
+  if (ndig <= 0 || ndig > maxdig || ndig > HB_MAXDIG) return hb_fail(HB_ERR_BAD_ARG, "%s: ndig=%d out of range", who, ndig);
+  bool any1 = false, anyk = false;
+  for (int t = 0; t < namt; t++) {
+    if (k[t] == 0 || k[t] >= c->m || h_gcd((long)k[t], (long)c->m) != 1) return hb_fail(HB_ERR_INDEX_SET, "automorph: k not in Zm*");
+    if (k[t] == 1) any1 = true; else anyk = true;
+  }
+  for (int i = 0; i < nS; i++) if (c->digit_of[S[i]] < 0) return hb_fail(HB_ERR_INDEX_SET, "%s: S must be a subset of the ctxt primes (prime %d)", who, S[i]);
+  if (any1 && !c1) return hb_fail(HB_ERR_BAD_ARG, "%s: c1 is required when some k == 1", who);
+  if (c1) HB_TRY(check_polys(c1, nitems, &c, "hb_hoisted_linear_map(c1)"));
+  HB_TRY(check_polys(digits, nitems * maxdig, &c, "hb_hoisted_linear_map(digits)"));
+  HB_TRY(check_polys(consts, namt, &c, "hb_hoisted_linear_map(consts)"));
+  HB_TRY(check_polys(acc0, nitems, &c, "hb_hoisted_linear_map(acc0)")); HB_TRY(check_polys(acc1, nitems, &c, "hb_hoisted_linear_map(acc1)"));
+  if (anyk && (!evk_a || !evk_b)) return hb_fail(HB_ERR_BAD_ARG, "%s: no key-switching matrices", who);
+  for (int t = 0; t < namt; t++) {
+    if (k[t] == 1) continue;
+    HB_TRY(check_polys(evk_a + (size_t)t * ndig, ndig, &c, "hb_hoisted_linear_map(evk_a)", true));
+    HB_TRY(check_polys(evk_b + (size_t)t * ndig, ndig, &c, "hb_hoisted_linear_map(evk_b)"));
+  }
+  // the accumulators are written while every other operand is still being read: they must be distinct and alias nothing
+  std::set<const hb_poly*> in, out;
+  in.insert(c0, c0 + nitems); in.insert(digits, digits + (size_t)nitems * maxdig); in.insert(consts, consts + namt);
+  if (c1) in.insert(c1, c1 + nitems);
+  for (int t = 0; t < namt; t++)
+    if (k[t] != 1) { in.insert(evk_a + (size_t)t * ndig, evk_a + (size_t)(t + 1) * ndig); in.insert(evk_b + (size_t)t * ndig, evk_b + (size_t)(t + 1) * ndig); }
+  out.insert(acc0, acc0 + nitems); out.insert(acc1, acc1 + nitems);
+  if ((int)out.size() != 2 * nitems) return hb_fail(HB_ERR_BAD_ARG, "%s: the accumulators must be distinct polynomials", who);
+  for (const hb_poly* p : out) if (in.count(p)) return hb_fail(HB_ERR_BAD_ARG, "%s: an accumulator aliases an input", who);
+  std::vector<int32_t> Sp(S, S + nS); Sp.insert(Sp.end(), c->special.begin(), c->special.end()); std::sort(Sp.begin(), Sp.end());
+  const int nSp = (int)Sp.size();
+  // every row a seeded matrix must regenerate is checked before anything is launched
+  bool seeded = false;
+  for (int t = 0; t < namt; t++)
+    for (int i = 0; k[t] != 1 && i < ndig; i++) {
+      const HbSeedSched* Q = evk_a[(size_t)t * ndig + i]->sched;
+      if (!Q) continue;
+      seeded = true;
+      for (int32_t r : Sp) if (!std::binary_search(Q->idx.begin(), Q->idx.end(), r)) return hb_fail(HB_ERR_INDEX_SET, "%s: row %d is not in the seeded set", who, r);
+    }
+  std::vector<u64> sc((size_t)nSp, 0);
+  for (int r = 0; r < nSp; r++)
+    if (std::find(S, S + nS, Sp[r]) != S + nS) sc[(size_t)r] = prod_mod(c, c->special.data(), (int)c->special.size(), c->q[Sp[r]]);
+  // amounts per launch; with seeded keys also per regeneration, whose scratch stays at HB_LINMAP_SEEDED polys
+  const int achunk = seeded ? std::max(1, HB_LINMAP_SEEDED / ndig) : HB_LINMAP_MAXAMT;
+  std::vector<hb_poly*> list, ka;
+  std::vector<int> slot;
+  for (int t0 = 0; t0 < namt; t0 += achunk) {
+    const int na = std::min(achunk, namt - t0);
+    list.clear(); slot.assign((size_t)na, -1);
+    for (int a = 0; a < na; a++)
+      if (k[t0 + a] != 1) { slot[(size_t)a] = (int)list.size(); list.insert(list.end(), evk_a + (size_t)(t0 + a) * ndig, evk_a + (size_t)(t0 + a + 1) * ndig); }
+    if (!list.empty()) HB_TRY(ks_expand_a(c, list.data(), (int)list.size(), Sp.data(), nSp, ka));
+    u64 item_rows = 0, shared_rows = 0;   // rows read per item and shared by the items, per row of the launch
+    for (int a = 0; a < na; a++) { item_rows += k[t0 + a] == 1 ? 2 : ndig + 1; shared_rows += k[t0 + a] == 1 ? 1 : 2 * ndig + 1; }
+    const bool acc = accumulate || t0 > 0;
+    HB_TRY(for_items(nitems, [&](int i0, int nit) {
+      for (int r0 = 0; r0 < nSp; r0 += HB_MAXROWS) {
+        const int nr = std::min(HB_MAXROWS, nSp - r0);
+        HbLinJob J; memset(&J, 0, sizeof(J));
+        J.N = c->N; J.m = c->m;
+        if (c->gen.on) { J.rep = c->gen.d_rep; J.irep = c->gen.d_irep; }
+        J.ndig = ndig; J.nitems = nit; J.namt = na; J.accumulate = acc ? 1 : 0;
+        fill_rows(J.rows, Sp.data() + r0, nr);
+        for (int i = 0; i < nr; i++) J.scal[i] = sc[(size_t)(r0 + i)];
+        for (int a = 0; a < na; a++) {
+          const int t = t0 + a;
+          J.k[a] = k[t]; J.cst[a] = consts[t]->d;
+          if (slot[(size_t)a] >= 0)
+            for (int i = 0; i < ndig; i++) { J.evk_a[a][i] = ka[(size_t)slot[(size_t)a] + i]->d; J.evk_b[a][i] = evk_b[(size_t)t * ndig + i]->d; }
+        }
+        for (int it = 0; it < nit; it++) {
+          J.c0[it] = c0[i0 + it]->d; J.c1[it] = c1 ? c1[i0 + it]->d : nullptr;
+          J.acc0[it] = acc0[i0 + it]->d; J.acc1[it] = acc1[i0 + it]->d;
+          for (int i = 0; i < ndig; i++) J.dig[it][i] = digits[(size_t)(i0 + it) * maxdig + i]->d;
+        }
+        const int ni = nit >= 4 ? 4 : nit >= 2 ? 2 : 1;
+        const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, (unsigned)((nit + ni - 1) / ni));
+        pre_launch(c);
+        switch (ni) {
+          case 1: HB_LAUNCH(k_ks_linmap<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+          case 2: HB_LAUNCH(k_ks_linmap<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+          default: HB_LAUNCH(k_ks_linmap<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+        }
+        // per item: its digit and c0 (or c0 and c1) rows per amount, two accumulators written (and read when accumulating);
+        // per launch: the key rows and the constant of every amount, once
+        HB_TRY(post_launch(c, "k_ks_linmap", ((item_rows + (acc ? 4 : 2)) * nit + shared_rows) * nr * c->N * 8));
+      }
+      return HB_OK;
+    }));
+  }
+  return HB_OK;
 }
 
 extern "C" int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1,

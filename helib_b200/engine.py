@@ -536,7 +536,28 @@ def _engine_hoist(cls):
         self._ck(self.lib.hb_automorph_keyswitch_digits(_arr(flat), nd, nd, len(digits), p, n, _arr(c0), C.c_uint64(int(k)),
                                                         _arr(evk_a), _arr(evk_b), _arr(out0), _arr(out1)))
 
+    def hoisted_linear_map(self, digits, S, c0, c1, ks, consts, evk_a, evk_b, acc0, acc1, accumulate=False):
+        """acc (+)= sum_j consts[j] * (hoisted automorph by ks[j]) over S | special, for every item (hb_hoisted_linear_map).
+        digits: per item, the digit Polys of c1; c1 may be None when no k is 1; evk_a / evk_b: per amount, the list of
+        ndig matrix Polys (None where k == 1)."""
+        a, p, n = _idx(S)
+        nd = len(digits[0])
+        flat = [d for item in digits for d in item]
+        kk = np.ascontiguousarray(np.array([int(x) for x in ks], dtype=np.uint64))
+        na = len(kk)
+
+        def keys(evk):
+            arr = (C.c_void_p * max(1, na * nd))()
+            for j, mat in enumerate(evk):
+                for i in range(nd):
+                    arr[j * nd + i] = mat[i].h if mat is not None else None
+            return arr
+        self._ck(self.lib.hb_hoisted_linear_map(_arr(flat), nd, nd, len(digits), p, n, _arr(c0), _arr(c1) if c1 is not None else None,
+                                                na, kk.ctypes.data_as(u64p), _arr(consts), keys(evk_a), keys(evk_b),
+                                                _arr(acc0), _arr(acc1), int(bool(accumulate))))
+
     cls.automorph_keyswitch_digits = automorph_keyswitch_digits
+    cls.hoisted_linear_map = hoisted_linear_map
     return cls
 
 

@@ -198,6 +198,24 @@ int hb_sub_div_by_primes(hb_poly* const* dst, hb_poly* const* src, int nitems, c
 int hb_automorph_keyswitch_digits(hb_poly* const* digits, int maxdig, int ndig, int nitems, const int32_t* S, int nS,
                                   hb_poly* const* c0, uint64_t k, hb_poly* const* evk_a, hb_poly* const* evk_b,
                                   hb_poly* const* out0, hb_poly* const* out1);
+/* Hoisted linear map (SURVEY 8f-1): the loop body of MatMul1DExec::mul's native FULL branch (src/matmul.cpp:1226-1252) for
+ * the amounts whose matrix is direct -- sum_j consts[j] * BasicAutomorphPrecon::automorph(k[j]) with the mod-down left lazy.
+ * digits = hb_break_into_digits of c1 over S (maxdig, ndig as for hb_automorph_keyswitch_digits); c0, c1 over S;
+ * consts[j] over S | special (evaluation form); evk_a/evk_b [namt*ndig], matrix j = entries j*ndig .. j*ndig+ndig-1, the
+ * matrix for s(X^k[j]) -> s (ignored, and may be NULL, where k[j] == 1).  Over S | special, for every item:
+ *   acc0 (+)= sum_j consts[j] * ( P*sigma_kj(c0) + [k_j != 1] sum_i sigma_kj(D_i)*b_{j,i} )
+ *   acc1 (+)= sum_j consts[j] * ( [k_j == 1] P*c1  +  [k_j != 1] sum_i sigma_kj(D_i)*a_{j,i} )
+ * P*x is addPrimesAndScale: x*P on the rows of S and 0 on the special rows.  accumulate = 0 overwrites acc0/acc1.
+ * The items share k, consts and the matrices.  Power-of-two and general m.  One k_ks_linmap launch per group of up to 64
+ * amounts (per item chunk and row chunk); seeded evk_a are regenerated a few matrices at a time, so the key scratch does
+ * not grow with namt.  Errors, all reported before any launch: k[j] not in Z_m^*, S not within the ctxt primes, or a
+ * seeded evk_a without a needed row -> HB_ERR_INDEX_SET; namt <= 0, ndig out of range, c1 NULL while some k[j] == 1, an
+ * accumulator aliasing an input or another accumulator, or a seeded handle other than in evk_a -> HB_ERR_BAD_ARG.
+ * Stream-ordered, no synchronisation; after the first call, a call of the same shape allocates nothing. */
+int hb_hoisted_linear_map(hb_poly* const* digits, int maxdig, int ndig, int nitems, const int32_t* S, int nS,
+                          hb_poly* const* c0, hb_poly* const* c1, int namt, const uint64_t* k, hb_poly* const* consts,
+                          hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* acc0, hb_poly* const* acc1,
+                          int accumulate);
 /* Ctxt::tensorProduct of two canonical 2-part ciphertexts (src/Ctxt.cpp:1563-1608) */
 int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1,
               hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int nitems, const int32_t* idx, int n);

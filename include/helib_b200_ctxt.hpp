@@ -827,6 +827,146 @@ class BasicAutomorphPrecon {
     if ((amt - k) % m != 0) result->smartAutomorph((long)(((unsigned __int128)(unsigned long)k * (unsigned long)Ctxt::invMod(amt, m)) % (unsigned long)m));
     return result;
   }
+  // The hoisted linear map of MatMul1DExec::mul's native FULL branch (src/matmul.cpp:1226-1252):
+  //   acc = 0;  for j: tmp = automorph(k[j]); tmp->multByConstant(*consts[j], sizes[j]); acc += *tmp;  return acc
+  // The amounts whose matrix is direct (getNextKSWmatrix(k).fromKey.powerOfX == k), and k == 1, are summed by one
+  // hb_hoisted_linear_map call over S | special, without intermediate ciphertexts; the rest, and a ciphertext with one
+  // part, take the loop above.  Bits and metadata are those of the loop.  BGV; CKKS: linearCombinationCKKS.
+  std::shared_ptr<Ctxt> linearCombination(const std::vector<long>& k, const std::vector<const DoubleCRT*>& consts, const std::vector<double>& sizes) const {
+    if (ctxt.isCKKS()) throw LogicError("linearCombination: use linearCombinationCKKS (explicit size, factor and rounding error)");
+    std::vector<Coef> cf;
+    for (size_t j = 0; j < consts.size(); j++) cf.push_back({consts[j], j < sizes.size() ? sizes[j] : -1.0, XD(), XD(), 0.0});
+    return combine(k, cf);
+  }
+  // CKKS: each constant's (size, factor, roundingErr) as multByConstantCKKS takes them.  Terms are fused when their matrix is
+  // direct, k != 1, and their factor equals the first such term's; if any term cannot be fused, every term takes the loop,
+  // because equalizeRationalFactors scales the partial sum it meets and that sum then depends on the order of the terms.
+  std::shared_ptr<Ctxt> linearCombinationCKKS(const std::vector<long>& k, const std::vector<const DoubleCRT*>& consts, const std::vector<XD>& sizes,
+                                              const std::vector<XD>& factors, const std::vector<double>& roundingErrs) const {
+    if (!ctxt.isCKKS()) throw LogicError("linearCombinationCKKS on a BGV ciphertext");
+    std::vector<Coef> cf;
+    for (size_t j = 0; j < consts.size(); j++) cf.push_back({consts[j], 0.0, sizes.at(j), factors.at(j), roundingErrs.at(j)});
+    return combine(k, cf);
+  }
+
+ private:
+  struct Coef { const DoubleCRT* c; double size; XD csize, factor; double err; };
+  void mulConst(Ctxt& t, const Coef& c) const {
+    if (ctxt.isCKKS()) t.multByConstantCKKS(*c.c, c.csize, c.factor, c.err); else t.multByConstant(*c.c, c.size);
+  }
+  // the metadata the loop's multByConstant / multByConstantCKKS gives a term (Ctxt::multByConstant returns early for a
+  // ciphertext without parts, so the metadata-only terms below are updated here)
+  void mulConstMeta(Ctxt& t, const Coef& c) const {
+    if (ctxt.isCKKS()) {
+      t.noiseBound = t.noiseBound * c.factor * c.csize + XD(c.err) * t.ratFactor * t.ptxtMag + t.noiseBound * XD(c.err);
+      t.ptxtMag = t.ptxtMag * c.csize;
+      t.ratFactor = t.ratFactor * c.factor;
+    } else {
+      const double size = c.size < 0.0 ? t.pubKey.noiseBoundForMod(t.ptxtSpace, t.context.getPhiM()) : c.size;
+      t.noiseBound = t.noiseBound * XD(size);
+    }
+  }
+  // Ctxt::modUpToSet / addCtxt on metadata only, for terms with one intFactor: f is what DoubleCRT::addPrimesAndScale returns
+  static void modUpMeta(Ctxt& c, const IndexSet& s) {
+    IndexSet d = s / c.primeSet;
+    if (empty(d)) return;
+    const double f = c.pubKey.logOfProduct(d);
+    c.noiseBound = c.noiseBound * XD::exp(f);
+    c.ratFactor = c.ratFactor * XD::exp(f);
+    c.primeSet.insert(d);
+  }
+  static void addMeta(Ctxt& a, bool& first, Ctxt o) {
+    if (first) { a = o; first = false; return; }
+    if (!a.isCKKS()) a.reducePtxtSpace(o.ptxtSpace);
+    if (a.ptxtSpace != o.ptxtSpace) o.reducePtxtSpace(a.ptxtSpace);
+    modUpMeta(a, o.primeSet);
+    modUpMeta(o, a.primeSet);
+    if (a.isCKKS()) Ctxt::equalizeRationalFactors(a, o, a.context.getR());
+    a.ptxtMag = a.ptxtMag + o.ptxtMag;
+    a.noiseBound = a.noiseBound + o.noiseBound;
+  }
+  std::shared_ptr<Ctxt> combine(const std::vector<long>& ks, const std::vector<Coef>& cf) const {
+    if (ks.size() != cf.size()) throw InvalidArgument("linearCombination: one constant per amount");
+    const Context& context = ctxt.context;
+    const KeyInfo& pubKey = ctxt.pubKey;
+    const long m = context.getM();
+    const size_t n = ks.size();
+    const bool ckks = ctxt.isCKKS();
+    auto term = [&](size_t j) { auto t = automorph(ks[j]); mulConst(*t, cf[j]); return t; };
+    auto loop = [&](std::vector<std::shared_ptr<Ctxt>>& done) {
+      auto acc = std::make_shared<Ctxt>(pubKey, ctxt.ptxtSpace);
+      for (size_t j = 0; j < n; j++) *acc += *(done[j] ? done[j] : term(j));
+      return acc;
+    };
+    std::vector<std::shared_ptr<Ctxt>> done(n);
+    // which amounts one call can sum
+    std::vector<long> kk(n);
+    std::vector<const KeySwitch*> W(n, nullptr);
+    std::vector<char> fuse(n, 0);
+    size_t nk = 0, nf = 0;
+    const long keyID = ctxt.getKeyID();
+    const Coef* first = nullptr;
+    for (size_t j = 0; j < n && ctxt.parts.size() == 2; j++) {
+      kk[j] = ((ks[j] % m) + m) % m;
+      if (kk[j] == 1) { fuse[j] = !ckks; continue; }
+      if (std::gcd(kk[j], m) != 1 || !pubKey.isReachable(kk[j], keyID)) continue;
+      const KeySwitch* w = pubKey.getNextKSWmatrix(kk[j], keyID);
+      if (w->fromKey.powerOfX != kk[j] || w->toKeyID != keyID) continue;
+      if (ckks && first && (first->factor < cf[j].factor || cf[j].factor < first->factor)) continue;
+      if (!first) first = &cf[j];
+      W[j] = w; fuse[j] = 1; nk++;
+    }
+    for (size_t j = 0; j < n; j++) nf += fuse[j];
+    if (nk == 0 || (ckks && nf < n)) return loop(done);
+    // the other terms first: summing the fused ones apart reorders additions, which is exact only for one intFactor
+    for (size_t j = 0; j < n; j++)
+      if (!fuse[j]) { done[j] = term(j); if (!ckks && done[j]->intFactor != ctxt.intFactor) return loop(done); }
+    // the fused terms: one call
+    const IndexSet full = ctxt.primeSet | context.getSpecialPrimes();
+    DoubleCRT a0(context, full), a1(context, full);
+    {
+      std::vector<hb_poly*> dg, cs, ea, eb;
+      std::vector<uint64_t> kv;
+      for (auto& d : polyDigits) dg.push_back(d.handle());
+      const size_t nd = polyDigits.size();
+      for (size_t j = 0; j < n; j++) {
+        if (!fuse[j]) continue;
+        kv.push_back((uint64_t)kk[j]); cs.push_back(cf[j].c->handle());
+        for (size_t i = 0; i < nd; i++) { ea.push_back(W[j] ? W[j]->aHandle(i) : nullptr); eb.push_back(W[j] ? W[j]->b[i].handle() : nullptr); }
+      }
+      hb_poly* c0[1] = {ctxt.parts[0].dcrt.handle()}; hb_poly* c1[1] = {ctxt.parts[1].dcrt.handle()};
+      hb_poly* o0[1] = {a0.handle()}; hb_poly* o1[1] = {a1.handle()};
+      auto S = ctxt.primeSet.vec();
+      check(hb_hoisted_linear_map(dg.data(), (int)nd, (int)nd, 1, S.data(), (int)S.size(), c0, c1, (int)kv.size(), kv.data(), cs.data(),
+                                  ea.data(), eb.data(), o0, o1, 0));
+    }
+    auto acc = std::make_shared<Ctxt>(pubKey, ctxt.ptxtSpace);
+    acc->primeSet = full;
+    acc->intFactor = ctxt.intFactor;
+    acc->parts.emplace_back(a0, SKHandle());
+    acc->parts.emplace_back(a1, ctxt.parts[1].skHandle);
+    for (size_t j = 0; j < n; j++) if (!fuse[j]) *acc += *done[j];   // data only: the metadata is replayed below
+    // metadata: the loop's, term by term in its order
+    Ctxt meta(pubKey, ctxt.ptxtSpace);
+    bool empty_acc = true;
+    for (size_t j = 0; j < n; j++) {
+      Ctxt t(pubKey, ctxt.ptxtSpace);
+      if (!fuse[j]) t = *done[j];
+      else {
+        if (kk[j] == 1) t = ctxt;
+        else {
+          t.noiseBound = noise; t.intFactor = ctxt.intFactor; t.primeSet = full;
+          if (ckks) { t.ptxtMag = ctxt.ptxtMag; t.ratFactor = ctxt.ratFactor * XD::exp(pubKey.logOfProduct(context.getSpecialPrimes())); }
+        }
+        mulConstMeta(t, cf[j]);
+      }
+      t.parts.clear();
+      addMeta(meta, empty_acc, t);
+    }
+    acc->primeSet = meta.primeSet; acc->ptxtSpace = meta.ptxtSpace; acc->noiseBound = meta.noiseBound;
+    acc->intFactor = meta.intFactor; acc->ratFactor = meta.ratFactor; acc->ptxtMag = meta.ptxtMag;
+    return acc;
+  }
 };
 
 // ---- SURVEY 8f-2: the steps either side of the path ------------------------------------------------------------
