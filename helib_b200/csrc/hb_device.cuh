@@ -806,6 +806,150 @@ __global__ void __launch_bounds__(HB_THREADS) k_ks_linmap(const HbPrimeDev* __re
   }
 }
 
+// BSGS giant steps (MatMul1DExec::mul's non-iterative BSGS branches, src/matmul.cpp:1022-1057, 1097-1142), first pass: for
+// every giant step t and item u of the launch, both parts of
+//   out[t][u] (+)= sigma_kt( scal_t * sum_b cst[t][b] * baby[u][b] )
+// sigma_k is applied on the write side: the thread of position j loads baby word j of every item once, uses it for all the
+// giant steps of the launch, and writes each sum to the position that sigma_k moves j to, pi_{k^-1}(j) (the inverse of
+// DoubleCRT::automorph's gather; kinv = k^-1 mod m).  Sums of up to HB_BSGS_MAXBABY products below 2^120 fit 128 bits and
+// are reduced once.
+#define HB_BSGS_MACW 8          // giant steps x items per launch (NT x NI): their 128-bit sums stay in registers
+#define HB_BSGS_CST 1024        // constant rows per launch (giant steps x baby steps)
+#define HB_BSGS_BABY 512        // baby rows per launch and part (items x baby steps)
+#define HB_BSGS_MAXBABY 240     // baby steps per launch
+struct HbBsgsMacJob {
+  u64 N, m;
+  const int* rep; const int* irep;   // general m; null: power-of-two m
+  int nb, nt, ni, accumulate;
+  HbRows rows;
+  u64 kinv[HB_BSGS_MACW];
+  u64 scal[HB_BSGS_MACW];
+  const u64* cst[HB_BSGS_CST];       // [t*nb + b]; null: a zero diagonal
+  const u64* baby0[HB_BSGS_BABY];    // [u*nb + b]
+  const u64* baby1[HB_BSGS_BABY];
+  u64* out0[HB_BSGS_MACW];           // [t*NI + u]
+  u64* out1[HB_BSGS_MACW];
+};
+template <int NI>
+__global__ void __launch_bounds__(HB_THREADS) k_bsgs_mac(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT HbBsgsMacJob J) {
+  constexpr int NT = HB_BSGS_MACW / NI;
+  const int pi = J.rows.prime[blockIdx.y];
+  const HbPrimeDev P = primes[pi];
+  const size_t N = (size_t)J.N;
+  const size_t off = (size_t)pi * N;
+  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < N; j += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = off + j;
+    u64 h0[NT][NI], l0[NT][NI], h1[NT][NI], l1[NT][NI];
+#pragma unroll
+    for (int t = 0; t < NT; t++)
+#pragma unroll
+      for (int u = 0; u < NI; u++) { h0[t][u] = 0; l0[t][u] = 0; h1[t][u] = 0; l1[t][u] = 0; }
+    for (int b = 0; b < J.nb; b++) {
+      u64 x0[NI], x1[NI];
+#pragma unroll
+      for (int u = 0; u < NI; u++) {
+        x0[u] = 0; x1[u] = 0;
+        if (u < J.ni) { x0[u] = J.baby0[u * J.nb + b][o]; x1[u] = J.baby1[u * J.nb + b][o]; }
+      }
+#pragma unroll
+      for (int t = 0; t < NT; t++) {
+        const u64* c = t < J.nt ? J.cst[t * J.nb + b] : nullptr;
+        if (!c) continue;
+        const u64 w = c[o];
+#pragma unroll
+        for (int u = 0; u < NI; u++) { hb_mac128(h0[t][u], l0[t][u], x0[u], w); hb_mac128(h1[t][u], l1[t][u], x1[u], w); }
+      }
+    }
+    const u64 rj = J.rep ? (u64)J.rep[j] : 2 * (u64)j + 1;   // m <= 2^20: rj*kinv < 2^40
+#pragma unroll
+    for (int t = 0; t < NT; t++) {
+      if (t < J.nt) {
+        const u64 kk = J.kinv[t];
+        const size_t g = off + (J.rep ? (size_t)J.irep[(rj * kk) % J.m] : (size_t)(((rj * kk) & (J.m - 1)) >> 1));
+        const u64 s = hb_reduce128(0, J.scal[t], P);
+#pragma unroll
+        for (int u = 0; u < NI; u++) {
+          if (u < J.ni) {
+            u64* d0 = J.out0[t * NI + u];
+            u64* d1 = J.out1[t * NI + u];
+            u64 v0 = hb_mulmod(hb_reduce128(h0[t][u], l0[t][u], P), s, P);
+            u64 v1 = hb_mulmod(hb_reduce128(h1[t][u], l1[t][u], P), s, P);
+            if (J.accumulate) { v0 = hb_addmod(v0, d0[g], P.q); v1 = hb_addmod(v1, d1[g], P.q); }
+            d0[g] = v0; d1[g] = v1;
+          }
+        }
+      }
+    }
+  }
+}
+
+// BSGS giant steps, last pass: the key switch of every rotated term (Ctxt::keySwitchPart after breakIntoDigits, with the
+// addPrimesAndScale of c0 folded in) and the unrotated terms, summed into the accumulators in one pass per group of terms:
+//   acc0 (+)= sum_t [rotated] ( P*x0_t + sum_i D_{t,i}*b_{t,i} )  +  [unrotated] scx*x0_t
+//   acc1 (+)= sum_t [rotated] (          sum_i D_{t,i}*a_{t,i} )  +  [unrotated] scx*x1_t
+// Every product is below 2^120 and is summed in 128 bits without reduction: the host keeps nt*(ndig+1) + 1 <= 255.
+// Term t of item it reads slot t*nitems + it.  grid = (coefficient blocks, rows, item groups of NI), as k_ks_linmap.
+#define HB_BSGS_GROUP 32        // giant steps x items per group: the scratch of rotated sums, mod-downs and digits
+struct HbGiantJob {
+  u64 N;
+  int ndig, nitems, nt, accumulate;
+  HbRows rows;
+  u64 scp[HB_MAXROWS];               // P mod q on the rows of S, 0 on the special rows (addPrimesAndScale)
+  u64 scx[HB_MAXROWS];               // the factor of an unrotated term: scp (baby steps over S) or 1 (over S | special)
+  unsigned char plain[HB_BSGS_GROUP];
+  const u64* evk_a[HB_BSGS_GROUP][HB_MAXDIG];
+  const u64* evk_b[HB_BSGS_GROUP][HB_MAXDIG];
+  const u64* x0[HB_BSGS_GROUP];
+  const u64* x1[HB_BSGS_GROUP];
+  const u64* dig[HB_BSGS_GROUP][HB_MAXDIG];
+  u64* acc0[HB_BSGS_GROUP];
+  u64* acc1[HB_BSGS_GROUP];
+};
+template <int NI>
+__global__ void __launch_bounds__(HB_THREADS) k_ks_giant(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT HbGiantJob J) {
+  const int pi = J.rows.prime[blockIdx.y];
+  const HbPrimeDev P = primes[pi];
+  const size_t N = (size_t)J.N;
+  const size_t off = (size_t)pi * N;
+  const u64 sp = J.scp[blockIdx.y], sx = J.scx[blockIdx.y];
+  const int it0 = blockIdx.z * NI;
+  const int cnt = J.nitems - it0 < NI ? J.nitems - it0 : NI;
+  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < N; j += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = off + j;
+    u64 h0[NI], l0[NI], h1[NI], l1[NI];
+#pragma unroll
+    for (int u = 0; u < NI; u++) {
+      h0[u] = 0; l0[u] = 0; h1[u] = 0; l1[u] = 0;
+      if (J.accumulate && u < cnt) { l0[u] = J.acc0[it0 + u][o]; l1[u] = J.acc1[it0 + u][o]; }
+    }
+    for (int t = 0; t < J.nt; t++) {
+      const int s0 = t * J.nitems + it0;
+      if (J.plain[t]) {
+        if (sx) {
+#pragma unroll
+          for (int u = 0; u < NI; u++)
+            if (u < cnt) { hb_mac128(h0[u], l0[u], J.x0[s0 + u][o], sx); hb_mac128(h1[u], l1[u], J.x1[s0 + u][o], sx); }
+        }
+        continue;
+      }
+      if (sp) {
+#pragma unroll
+        for (int u = 0; u < NI; u++)
+          if (u < cnt) hb_mac128(h0[u], l0[u], J.x0[s0 + u][o], sp);
+      }
+      for (int i = 0; i < J.ndig; i++) {
+        const u64 b = J.evk_b[t][i][o], a = J.evk_a[t][i][o];
+#pragma unroll
+        for (int u = 0; u < NI; u++)
+          if (u < cnt) { const u64 d = J.dig[s0 + u][i][o]; hb_mac128(h0[u], l0[u], d, b); hb_mac128(h1[u], l1[u], d, a); }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < NI; u++)
+      if (u < cnt) { J.acc0[it0 + u][o] = hb_reduce128(h0[u], l0[u], P); J.acc1[it0 + u][o] = hb_reduce128(h1[u], l1[u], P); }
+  }
+}
+
 
 // ------------------------------------------------------------------------------------------
 // Canonical-embedding norm (noise metadata): max_j |f(zeta^(2j+1))|, zeta = e^(i*pi/N), in FP64.

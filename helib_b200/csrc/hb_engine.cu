@@ -120,6 +120,7 @@ struct hb_ctx {
   size_t prg_start_cap = 0, prg_off_cap = 0;
   int prg_window = 0;   // HB_PRG_WINDOW=w: count w buffers per row in parallel instead of the statistical bound (tests the slow path)
   std::vector<hb_poly*> ks_a;   // a_i regenerated from a seeded evk_a for the key switch in flight (allocated on first use)
+  std::vector<hb_poly*> bsgs;   // hb_bsgs_linear_map: rotated sums and their digits, HB_BSGS_GROUP*(2+ndig) polys (first use)
 };
 // The row schedule of a seeded set (hb_poly_create_seeded): the ChaCha20 key, the rows, and in one device allocation the
 // first buffer of every schedule row (start[T+1]) and the exclusive row offset of every counted buffer (off[T*wmax]).
@@ -347,6 +348,7 @@ extern "C" void hb_ctx_destroy(hb_ctx* c) {
   cudaFree(c->tmpA); cudaFree(c->tmpB); cudaFree(c->d_tw); cudaFree(c->d_primes); cudaFree(c->d_stats);
   cudaFree(c->prg_start); cudaFree(c->prg_off); cudaFree(c->prg_ticket);
   for (hb_poly* p : c->ks_a) { cudaFree(p->d); delete p; }
+  for (hb_poly* p : c->bsgs) { cudaFree(p->d); delete p; }
   for (HbTmap* sl : c->tmap_slabs) cudaFree(sl);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
   delete c;
@@ -2305,6 +2307,245 @@ extern "C" int hb_hoisted_linear_map(hb_poly* const* digits, int maxdig, int ndi
       }
       return HB_OK;
     }));
+  }
+  return HB_OK;
+}
+
+// BSGS linear map (SURVEY 8f-1): the giant-step phase of MatMul1DExec::mul's non-iterative BSGS branches (src/matmul.cpp:
+// 1022-1057 native, 1097-1142 bad dimension).  Work goes in groups of at most HB_BSGS_GROUP (giant step, item) pairs, so the
+// scratch is HB_BSGS_GROUP*(2+ndig) polys whatever the number of giant steps.  Per group: k_bsgs_mac forms the rotated
+// inner sums, the extended form's mod-down and breakIntoDigits run once over all of the group's rotated sums, and
+// k_ks_giant key-switches and sums them into the accumulators.
+static int bsgs_impl(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, int nitems, const int32_t* S, int nS, int extended,
+                     uint64_t ptxt_space, int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
+                     hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk, hb_poly* const* acc0, hb_poly* const* acc1,
+                     int accumulate, double* norms);
+extern "C" int hb_bsgs_linear_map(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, int nitems,
+                                  const int32_t* S, int nS, int extended, uint64_t ptxt_space,
+                                  int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
+                                  hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk,
+                                  hb_poly* const* acc0, hb_poly* const* acc1, int accumulate) {
+  return bsgs_impl(baby0, baby1, nbaby, nitems, S, nS, extended, ptxt_space, ngiant, kgiant, consts, scal, evk_a, evk_b, ndig_evk,
+                   acc0, acc1, accumulate, nullptr);
+}
+// norms[(item*ngiant + t)*(HB_MAXDIG + 2) + i]: ln ||E_i|| of the digits of rotated giant step t (i < ndig), then ||delta/P||
+// of its two parts' mod-down (extended form) -- what keySwitchPart and modDownToSet add to the noise bound
+extern "C" int hb_bsgs_linear_map_norm(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, int nitems,
+                                       const int32_t* S, int nS, int extended, uint64_t ptxt_space,
+                                       int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
+                                       hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk,
+                                       hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms) {
+  if (!norms) return hb_fail(HB_ERR_BAD_ARG, "hb_bsgs_linear_map_norm: null output");
+  return bsgs_impl(baby0, baby1, nbaby, nitems, S, nS, extended, ptxt_space, ngiant, kgiant, consts, scal, evk_a, evk_b, ndig_evk,
+                   acc0, acc1, accumulate, norms);
+}
+static int bsgs_impl(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, int nitems, const int32_t* S, int nS, int extended,
+                     uint64_t ptxt_space, int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
+                     hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk, hb_poly* const* acc0, hb_poly* const* acc1,
+                     int accumulate, double* norms) {
+  static const char* who = "hb_bsgs_linear_map";
+  hb_ctx* c = nullptr;
+  if (nbaby <= 0 || nitems <= 0 || ngiant <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: nbaby, nitems and ngiant must be positive", who);
+  if (extended != 0 && extended != 1) return hb_fail(HB_ERR_BAD_ARG, "%s: extended must be 0 or 1", who);
+  if (!kgiant || !consts) return hb_fail(HB_ERR_BAD_ARG, "%s: no giant steps", who);
+  HB_TRY(check_polys(baby0, nitems * nbaby, &c, "hb_bsgs_linear_map(baby0)"));
+  HB_TRY(check_polys(baby1, nitems * nbaby, &c, "hb_bsgs_linear_map(baby1)"));
+  HB_TRY(check_idx(c, S, nS, who));
+  if (ptxt_space < 1) return hb_fail(HB_ERR_BAD_ARG, "%s: ptxt_space must be at least 1", who);
+  if (c->special.empty()) return hb_fail(HB_ERR_BAD_ARG, "%s: context has no special primes", who);
+  for (int i = 0; i < nS; i++) if (c->digit_of[S[i]] < 0) return hb_fail(HB_ERR_INDEX_SET, "%s: S must be a subset of the ctxt primes (prime %d)", who, S[i]);
+  bool anyk = false;
+  for (int t = 0; t < ngiant; t++) {
+    if (kgiant[t] == 0 || kgiant[t] >= c->m || h_gcd((long)kgiant[t], (long)c->m) != 1) return hb_fail(HB_ERR_INDEX_SET, "automorph: k not in Zm*");
+    if (kgiant[t] != 1) anyk = true;
+    // reLinearize applies relin_CKKS_adjust after the mod-down (src/Ctxt.cpp:733-736), which a factor folded into the sum
+    // would precede; it is 1 for BGV, whose bad dimensions are the extended form's callers
+    if (extended && scal && scal[t] != 1) return hb_fail(HB_ERR_BAD_ARG, "%s: scal must be 1 in the extended form", who);
+  }
+  for (int i = 0; i < ngiant * nbaby; i++) if (consts[i]) HB_TRY(check_polys(consts + i, 1, &c, "hb_bsgs_linear_map(consts)"));
+  HB_TRY(check_polys(acc0, nitems, &c, "hb_bsgs_linear_map(acc0)")); HB_TRY(check_polys(acc1, nitems, &c, "hb_bsgs_linear_map(acc1)"));
+  // the digits of S (src/DoubleCRT.cpp:485-493)
+  int nd = 0;
+  {
+    std::vector<char> rem(c->nprimes, 0); int left = nS;
+    for (int i = 0; i < nS; i++) rem[S[i]] = 1;
+    for (; left > 0; nd++) for (int i = 0; i < c->nprimes; i++) if (rem[i] && c->digit_of[i] == nd) { rem[i] = 0; left--; }
+  }
+  if (anyk) {
+    if (nd > ndig_evk || nd > HB_MAXDIG) return hb_fail(HB_ERR_BAD_ARG, "%s: key-switching matrices have %d columns, need %d", who, ndig_evk, nd);
+    if (!evk_a || !evk_b) return hb_fail(HB_ERR_BAD_ARG, "%s: no key-switching matrices", who);
+    for (int t = 0; t < ngiant; t++) {
+      if (kgiant[t] == 1) continue;
+      HB_TRY(check_polys(evk_a + (size_t)t * ndig_evk, nd, &c, "hb_bsgs_linear_map(evk_a)", true));
+      HB_TRY(check_polys(evk_b + (size_t)t * ndig_evk, nd, &c, "hb_bsgs_linear_map(evk_b)"));
+    }
+  }
+  // the accumulators are written while every other operand is still being read: they must be distinct and alias nothing
+  std::set<const hb_poly*> in, out;
+  in.insert(baby0, baby0 + (size_t)nitems * nbaby); in.insert(baby1, baby1 + (size_t)nitems * nbaby);
+  for (int i = 0; i < ngiant * nbaby; i++) if (consts[i]) in.insert(consts[i]);
+  for (int t = 0; t < ngiant; t++)
+    if (kgiant[t] != 1) { in.insert(evk_a + (size_t)t * ndig_evk, evk_a + (size_t)t * ndig_evk + nd); in.insert(evk_b + (size_t)t * ndig_evk, evk_b + (size_t)t * ndig_evk + nd); }
+  out.insert(acc0, acc0 + nitems); out.insert(acc1, acc1 + nitems);
+  if ((int)out.size() != 2 * nitems) return hb_fail(HB_ERR_BAD_ARG, "%s: the accumulators must be distinct polynomials", who);
+  for (const hb_poly* p : out) if (in.count(p)) return hb_fail(HB_ERR_BAD_ARG, "%s: an accumulator aliases an input", who);
+  std::vector<int32_t> Sp(S, S + nS); Sp.insert(Sp.end(), c->special.begin(), c->special.end()); std::sort(Sp.begin(), Sp.end());
+  const int nSp = (int)Sp.size();
+  bool seeded = false;
+  for (int t = 0; t < ngiant; t++)
+    for (int i = 0; kgiant[t] != 1 && i < nd; i++) {
+      const HbSeedSched* Q = evk_a[(size_t)t * ndig_evk + i]->sched;
+      if (!Q) continue;
+      seeded = true;
+      for (int32_t r : Sp) if (!std::binary_search(Q->idx.begin(), Q->idx.end(), r)) return hb_fail(HB_ERR_INDEX_SET, "%s: row %d is not in the seeded set", who, r);
+    }
+  // ---- every argument is checked: nothing was launched before this point
+  std::vector<u64> scp((size_t)nSp, 0), scx((size_t)nSp, 1);
+  for (int r = 0; r < nSp; r++) {
+    if (std::find(S, S + nS, Sp[r]) != S + nS) scp[(size_t)r] = prod_mod(c, c->special.data(), (int)c->special.size(), c->q[Sp[r]]);
+    if (!extended) scx[(size_t)r] = scp[(size_t)r];
+  }
+  std::vector<u64> kinv((size_t)ngiant);
+  for (int t = 0; t < ngiant; t++) h_invmod(kgiant[t], c->m, &kinv[(size_t)t]);
+  const std::vector<int32_t> R = extended ? Sp : std::vector<int32_t>(S, S + nS);   // the rows of the baby steps
+  const int nR = (int)R.size();
+  // scratch: slot s of a group holds the rotated sum (x0, x1) of one (giant step, item) and its nd digits
+  const int G = std::min(HB_BSGS_GROUP, nitems * ngiant);   // a group never holds more pairs than the call has
+  while ((int)c->bsgs.size() < G * (2 + nd)) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->bsgs.push_back(p); }
+  hb_poly* const* X0 = c->bsgs.data();
+  hb_poly* const* X1 = X0 + G;
+  hb_poly* const* DG = X0 + 2 * G;
+  const int ic = std::min(nitems, G);                 // items per group
+  const int gg = std::max(1, G / ic);                 // giant steps per group
+  const int NI = ic >= 4 ? 4 : ic >= 2 ? 2 : 1, NT = HB_BSGS_MACW / NI;
+  const int nbl = std::min(HB_BSGS_MAXBABY, std::min(HB_BSGS_CST / NT, HB_BSGS_BABY / NI));   // baby steps per k_bsgs_mac launch
+  // terms per k_ks_giant launch: the 128-bit budget, and with seeded keys the key scratch (HB_LINMAP_SEEDED polys)
+  const int tmax = std::max(1, std::min(254 / (nd + 1), seeded ? HB_LINMAP_SEEDED / std::max(1, nd) : G));
+  bool acc_on = accumulate != 0;
+  std::vector<hb_poly*> rot0, rot01, rdig, list, ka;
+  for (int i0 = 0; i0 < nitems; i0 += ic) {
+    const int nit = std::min(ic, nitems - i0);
+    acc_on = accumulate != 0;
+    for (int t0 = 0; t0 < ngiant; t0 += gg) {
+      const int ng = std::min(gg, ngiant - t0);
+      // 1. the rotated inner sums of the group: slot a*nit + it
+      for (int u0 = 0; u0 < nit; u0 += NI) {
+        const int ni = std::min(NI, nit - u0);
+        for (int a0 = 0; a0 < ng; a0 += NT) {
+          const int nt = std::min(NT, ng - a0);
+          for (int b0 = 0; b0 < nbaby; b0 += nbl) {
+            const int nb = std::min(nbl, nbaby - b0);
+            for (int r0 = 0; r0 < nR; r0 += HB_MAXROWS) {
+              const int nr = std::min(HB_MAXROWS, nR - r0);
+              HbBsgsMacJob J; memset(&J, 0, sizeof(J));
+              J.N = c->N; J.m = c->m;
+              if (c->gen.on) { J.rep = c->gen.d_rep; J.irep = c->gen.d_irep; }
+              J.nb = nb; J.nt = nt; J.ni = ni; J.accumulate = b0 > 0;
+              fill_rows(J.rows, R.data() + r0, nr);
+              u64 ncst = 0;
+              for (int a = 0; a < nt; a++) {
+                const int t = t0 + a0 + a;
+                J.kinv[a] = kinv[(size_t)t]; J.scal[a] = scal ? scal[t] : 1;
+                for (int b = 0; b < nb; b++) {
+                  hb_poly* cp = consts[(size_t)t * nbaby + b0 + b];
+                  J.cst[a * nb + b] = cp ? cp->d : nullptr;
+                  ncst += cp != nullptr;
+                }
+                for (int u = 0; u < ni; u++) {
+                  const int s = (a0 + a) * nit + u0 + u;
+                  J.out0[a * NI + u] = X0[s]->d; J.out1[a * NI + u] = X1[s]->d;
+                }
+              }
+              for (int u = 0; u < ni; u++)
+                for (int b = 0; b < nb; b++) {
+                  const size_t e = (size_t)(i0 + u0 + u) * nbaby + b0 + b;
+                  J.baby0[u * nb + b] = baby0[e]->d; J.baby1[u * nb + b] = baby1[e]->d;
+                }
+              const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, 1);
+              pre_launch(c);
+              switch (NI) {
+                case 1: HB_LAUNCH(k_bsgs_mac<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+                case 2: HB_LAUNCH(k_bsgs_mac<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+                default: HB_LAUNCH(k_bsgs_mac<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+              }
+              // the baby rows of the items and the constant rows of the giant steps once; two sums written per pair
+              // (and read when a later baby chunk adds to them)
+              HB_TRY(post_launch(c, "k_bsgs_mac", ((u64)2 * ni * nb + ncst + (u64)(b0 > 0 ? 4 : 2) * ni * nt) * nr * c->N * 8));
+            }
+          }
+        }
+      }
+      // 2. the rotated sums' mod-down (extended form) and digits, batched over the group
+      rot0.clear(); rot01.clear(); rdig.clear();
+      for (int a = 0; a < ng; a++) {
+        if (kgiant[t0 + a] == 1) continue;
+        for (int it = 0; it < nit; it++) {
+          const int s = a * nit + it;
+          rot0.push_back(X1[s]); rot01.push_back(X0[s]); rot01.push_back(X1[s]);
+          for (int i = 0; i < nd; i++) rdig.push_back(DG[(size_t)s * nd + i]);
+        }
+      }
+      if (!rot0.empty()) {
+        std::vector<double> sdn(norms && extended ? rot01.size() : 0), ldn(norms ? rdig.size() : 0);
+        if (extended) HB_TRY(scale_down_impl(rot01.data(), (int)rot01.size(), Sp.data(), nSp, S, nS, ptxt_space, norms ? sdn.data() : nullptr));
+        int ndo = 0;
+        HB_TRY(break_into_digits_impl(rot0.data(), (int)rot0.size(), S, nS, rdig.data(), nd, &ndo, norms ? ldn.data() : nullptr));
+        for (int a = 0, r = 0; norms && a < ng; a++) {
+          if (kgiant[t0 + a] == 1) continue;
+          for (int it = 0; it < nit; it++, r++) {
+            double* o = norms + ((size_t)(i0 + it) * ngiant + t0 + a) * (HB_MAXDIG + 2);
+            for (int i = 0; i < nd; i++) o[i] = ldn[(size_t)r * nd + i];
+            if (extended) { o[HB_MAXDIG] = sdn[(size_t)2 * r]; o[HB_MAXDIG + 1] = sdn[(size_t)2 * r + 1]; }
+          }
+        }
+      }
+      // 3. key switch and sum, tmax terms per launch
+      for (int a0 = 0; a0 < ng;) {
+        int nt = 0, nrot = 0;
+        while (a0 + nt < ng && nt < tmax) { nrot += kgiant[t0 + a0 + nt] != 1; nt++; if (seeded && (nrot + 1) * nd > HB_LINMAP_SEEDED) break; }
+        list.clear();
+        for (int a = 0; a < nt; a++) {
+          const int t = t0 + a0 + a;
+          if (kgiant[t] != 1) list.insert(list.end(), evk_a + (size_t)t * ndig_evk, evk_a + (size_t)t * ndig_evk + nd);
+        }
+        if (!list.empty()) HB_TRY(ks_expand_a(c, list.data(), (int)list.size(), Sp.data(), nSp, ka));
+        u64 item_rows = 0, key_rows = 0;   // rows read per item and shared by the items, per row of the launch
+        for (int r0 = 0; r0 < nSp; r0 += HB_MAXROWS) {
+          const int nr = std::min(HB_MAXROWS, nSp - r0);
+          HbGiantJob J; memset(&J, 0, sizeof(J));
+          J.N = c->N; J.ndig = nd; J.nitems = nit; J.nt = nt; J.accumulate = acc_on ? 1 : 0;
+          fill_rows(J.rows, Sp.data() + r0, nr);
+          for (int i = 0; i < nr; i++) { J.scp[i] = scp[(size_t)(r0 + i)]; J.scx[i] = scx[(size_t)(r0 + i)]; }
+          item_rows = 0; key_rows = 0;
+          for (int a = 0, slot = 0; a < nt; a++) {
+            const int t = t0 + a0 + a;
+            J.plain[a] = kgiant[t] == 1;
+            if (!J.plain[a]) {
+              for (int i = 0; i < nd; i++) { J.evk_a[a][i] = ka[(size_t)slot * nd + i]->d; J.evk_b[a][i] = evk_b[(size_t)t * ndig_evk + i]->d; }
+              slot++;
+            }
+            item_rows += J.plain[a] ? 2 : nd + 1; key_rows += J.plain[a] ? 0 : 2 * nd;
+            for (int it = 0; it < nit; it++) {
+              const int s = (a0 + a) * nit + it, sl = a * nit + it;
+              J.x0[sl] = X0[s]->d; J.x1[sl] = X1[s]->d;
+              for (int i = 0; i < nd && !J.plain[a]; i++) J.dig[sl][i] = DG[(size_t)s * nd + i]->d;
+            }
+          }
+          for (int it = 0; it < nit; it++) { J.acc0[it] = acc0[i0 + it]->d; J.acc1[it] = acc1[i0 + it]->d; }
+          const int ni = nit >= 4 ? 4 : nit >= 2 ? 2 : 1;
+          const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, (unsigned)((nit + ni - 1) / ni));
+          pre_launch(c);
+          switch (ni) {
+            case 1: HB_LAUNCH(k_ks_giant<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+            case 2: HB_LAUNCH(k_ks_giant<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+            default: HB_LAUNCH(k_ks_giant<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+          }
+          HB_TRY(post_launch(c, "k_ks_giant", ((item_rows + (acc_on ? 4 : 2)) * nit + key_rows) * nr * c->N * 8));
+        }
+        acc_on = true;
+        a0 += nt;
+      }
+    }
   }
   return HB_OK;
 }

@@ -556,8 +556,33 @@ def _engine_hoist(cls):
                                                 na, kk.ctypes.data_as(u64p), _arr(consts), keys(evk_a), keys(evk_b),
                                                 _arr(acc0), _arr(acc1), int(bool(accumulate))))
 
+    def bsgs_linear_map(self, baby0, baby1, S, ks, consts, evk_a, evk_b, acc0, acc1, extended=False, ptxt_space=1,
+                        scal=None, accumulate=False):
+        """acc (+)= the giant steps of a BSGS linear map over S | special, for every item (hb_bsgs_linear_map).
+        baby0 / baby1: per item, the list of the baby steps' parts; consts: per giant step, one Poly (or None) per baby
+        step; ks: the giant amounts; evk_a / evk_b: per giant step, the list of matrix Polys (None where k == 1)."""
+        a, p, n = _idx(S)
+        nb = len(baby0[0])
+        kk = np.ascontiguousarray(np.array([int(x) for x in ks], dtype=np.uint64))
+        ng = len(kk)
+        nd = max([len(m_) for m_ in evk_a if m_ is not None] or [1])
+        cs = (C.c_void_p * (ng * nb))(*[c_.h if c_ is not None else None for row in consts for c_ in row])
+
+        def keys(evk):
+            arr = (C.c_void_p * (ng * nd))()
+            for j, mat in enumerate(evk):
+                for i in range(nd):
+                    arr[j * nd + i] = mat[i].h if mat is not None else None
+            return arr
+        sc = np.ascontiguousarray(np.array([int(x) for x in scal], dtype=np.uint64)) if scal is not None else None
+        self._ck(self.lib.hb_bsgs_linear_map(_arr([x for it in baby0 for x in it]), _arr([x for it in baby1 for x in it]), nb, len(baby0),
+                                             p, n, int(bool(extended)), C.c_uint64(int(ptxt_space)), ng, kk.ctypes.data_as(u64p), cs,
+                                             sc.ctypes.data_as(u64p) if sc is not None else None, keys(evk_a), keys(evk_b), nd,
+                                             _arr(acc0), _arr(acc1), int(bool(accumulate))))
+
     cls.automorph_keyswitch_digits = automorph_keyswitch_digits
     cls.hoisted_linear_map = hoisted_linear_map
+    cls.bsgs_linear_map = bsgs_linear_map
     return cls
 
 

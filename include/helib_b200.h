@@ -216,6 +216,43 @@ int hb_hoisted_linear_map(hb_poly* const* digits, int maxdig, int ndig, int nite
                           hb_poly* const* c0, hb_poly* const* c1, int namt, const uint64_t* k, hb_poly* const* consts,
                           hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* acc0, hb_poly* const* acc1,
                           int accumulate);
+/* BSGS linear map (SURVEY 8f-1): the giant-step phase of MatMul1DExec::mul's non-iterative baby-step/giant-step branches
+ * (src/matmul.cpp:1022-1057 native, 1097-1142 bad dimension with ALT_MATMUL).  The baby steps are inputs:
+ * baby0/baby1[item*nbaby + j] are the two parts of baby step j of each item, over S (extended == 0: cleaned, the native
+ * branch) or over S | special (extended == 1: not cleaned, the bad-dimension branch, whose baby steps j = 0 the caller first
+ * brings to S | special with hb_add_primes_and_scale).  consts[t*nbaby + j] over the rows of the baby steps (NULL: a zero
+ * diagonal, skipped as MulAdd skips it), kgiant[t] the amount of giant step t, scal[t] an integer factor (NULL: all 1).
+ * For every item, with inner_t = scal[t] * sum_j consts[t*nbaby + j] * baby_j (both parts), over S | special:
+ *   kgiant[t] == 1: term_t = P*inner_t (extended == 0, addPrimesAndScale) or inner_t (extended == 1)
+ *   otherwise the steps of smartAutomorph(kgiant[t]) in HElib's order: sigma_k; if extended, the mod-down to S
+ *     (scaleDownToSet with ptxt_space, as reLinearize's dropSmallAndSpecialPrimes); breakIntoDigits of part 1 over S; the
+ *     key switch with matrix t: term_t = (P*c0' + sum_i D_i*b_{t,i}, sum_i D_i*a_{t,i})
+ *   acc0/acc1 (+)= sum_t term_t                                  (accumulate = 0 overwrites)
+ * scal[t] is relin_CKKS_adjust's factor, which HElib applies after the mod-down: it must be 1 when extended == 1.
+ * evk_a/evk_b [ngiant*ndig_evk], matrix t = entries t*ndig_evk .. (ignored, and may be NULL, where kgiant[t] == 1); the
+ * matrices need as many columns as S has digits.  ptxt_space = 1 for CKKS.  The items share the constants, amounts and
+ * matrices.  Power-of-two and general m; expanded or seeded evk_a.  Work goes in groups of at most 32 (giant step, item)
+ * pairs: one k_bsgs_mac pass per group and 8 pairs forms the rotated inner sums, the mod-down and digits run once per group
+ * over all of its rotated sums, and one k_ks_giant pass per group sums the key switches into the accumulators.  The
+ * scratch is min(32, nitems*ngiant)*(2 + ndig) polys whatever ngiant is.  Errors, all reported before any launch: kgiant[t] not in Z_m^*, S
+ * not within the ctxt primes, or a seeded evk_a without a needed row -> HB_ERR_INDEX_SET; counts out of range, too few
+ * matrix columns, scal != 1 in the extended form, an accumulator aliasing an input or another accumulator, or a seeded
+ * handle other than in evk_a -> HB_ERR_BAD_ARG.  Stream-ordered, no synchronisation; after the first call, a call of the
+ * same shape allocates nothing. */
+int hb_bsgs_linear_map(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, int nitems,
+                       const int32_t* S, int nS, int extended, uint64_t ptxt_space,
+                       int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
+                       hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk,
+                       hb_poly* const* acc0, hb_poly* const* acc1, int accumulate);
+/* The same, returning the norms the noise bookkeeping of smartAutomorph needs for every rotated giant step:
+ * norms[(item*ngiant + t)*(8 + 2) + i] = ln ||E_i|| of digit i (i < ndig; breakIntoDigits' norms), and at offsets 8 and 9 the
+ * ||delta/P|| of parts 0 and 1 of the extended form's mod-down (hb_scale_down_norm).  Entries of unrotated giant steps are not
+ * written.  Synchronises (host values). */
+int hb_bsgs_linear_map_norm(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, int nitems,
+                            const int32_t* S, int nS, int extended, uint64_t ptxt_space,
+                            int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
+                            hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk,
+                            hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms);
 /* Ctxt::tensorProduct of two canonical 2-part ciphertexts (src/Ctxt.cpp:1563-1608) */
 int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1,
               hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int nitems, const int32_t* idx, int n);

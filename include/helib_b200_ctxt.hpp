@@ -849,15 +849,15 @@ class BasicAutomorphPrecon {
     return combine(k, cf);
   }
 
- private:
+  // a constant as multByConstant (BGV: size, < 0 for the default) or multByConstantCKKS (csize, factor, err) takes it
   struct Coef { const DoubleCRT* c; double size; XD csize, factor; double err; };
-  void mulConst(Ctxt& t, const Coef& c) const {
-    if (ctxt.isCKKS()) t.multByConstantCKKS(*c.c, c.csize, c.factor, c.err); else t.multByConstant(*c.c, c.size);
+  static void mulConst(Ctxt& t, const Coef& c) {
+    if (t.isCKKS()) t.multByConstantCKKS(*c.c, c.csize, c.factor, c.err); else t.multByConstant(*c.c, c.size);
   }
   // the metadata the loop's multByConstant / multByConstantCKKS gives a term (Ctxt::multByConstant returns early for a
   // ciphertext without parts, so the metadata-only terms below are updated here)
-  void mulConstMeta(Ctxt& t, const Coef& c) const {
-    if (ctxt.isCKKS()) {
+  static void mulConstMeta(Ctxt& t, const Coef& c) {
+    if (t.isCKKS()) {
       t.noiseBound = t.noiseBound * c.factor * c.csize + XD(c.err) * t.ratFactor * t.ptxtMag + t.noiseBound * XD(c.err);
       t.ptxtMag = t.ptxtMag * c.csize;
       t.ratFactor = t.ratFactor * c.factor;
@@ -885,6 +885,7 @@ class BasicAutomorphPrecon {
     a.ptxtMag = a.ptxtMag + o.ptxtMag;
     a.noiseBound = a.noiseBound + o.noiseBound;
   }
+ private:
   std::shared_ptr<Ctxt> combine(const std::vector<long>& ks, const std::vector<Coef>& cf) const {
     if (ks.size() != cf.size()) throw InvalidArgument("linearCombination: one constant per amount");
     const Context& context = ctxt.context;
@@ -968,6 +969,190 @@ class BasicAutomorphPrecon {
     return acc;
   }
 };
+
+// ---- MatMul1DExec::mul's non-iterative baby-step/giant-step branches (src/matmul.cpp:989-1142) ------------------------
+// genToPow(dim, e) of a dimension with generator gen: gen^e mod m, a negative e through the inverse
+inline long genToPow(long gen, long e, long m) {
+  unsigned long b = (unsigned long)(e < 0 ? Ctxt::invMod(gen, m) : ((gen % m) + m) % m), r = 1, x = (unsigned long)(e < 0 ? -e : e);
+  for (; x; x >>= 1) { if (x & 1) r = (unsigned long)(((unsigned __int128)r * b) % (unsigned long)m); b = (unsigned long)(((unsigned __int128)b * b) % (unsigned long)m); }
+  return (long)r;
+}
+// GenBabySteps (src/matmul.cpp:925-980), its hoisted branch: v[j] = automorph(gen^j) of one BasicAutomorphPrecon, cleaned if asked
+inline std::vector<std::shared_ptr<Ctxt>> GenBabySteps(const Ctxt& ctxt, long gen, long g, bool clean) {
+  std::vector<std::shared_ptr<Ctxt>> v((size_t)g);
+  if (g == 1) { v[0] = std::make_shared<Ctxt>(ctxt); if (clean) v[0]->cleanUp(); return v; }
+  BasicAutomorphPrecon precon(ctxt);
+  for (long j = 0; j < g; j++) { v[(size_t)j] = precon.automorph(genToPow(gen, j, ctxt.context.getM())); if (clean) v[(size_t)j]->cleanUp(); }
+  return v;
+}
+// A diagonal of the matrix as MatMul1DExec's cache holds it: c == nullptr is a zero diagonal (MulAdd skips it); BGV takes
+// size (< 0: the default of multByConstant), CKKS csize, factor and err (multByConstantCKKS).
+using BsgsDiag = BasicAutomorphPrecon::Coef;
+// hb_bsgs_linear_map_norm: per giant step, 8 digit log-norms then the two mod-down norms
+constexpr long kNormStride8 = 8;
+// MatMul1DExec::mul for a dimension of size D > HELIB_KEYSWITCH_THRESH with generator gen, not iterative: ctxt becomes
+// sum_i cache[i] * rot_i(ctxt) (+ cache1[i] * rot_{i-D}(ctxt) for a bad dimension, cache1 non-empty).  g = KSGiantStepSize(D).
+// The baby steps are built as GenBabySteps builds them; every giant step is then summed by one hb_bsgs_linear_map call,
+// with the loop's bits and its metadata (noise, factors, prime set), replayed from the norms the call returns.  The loop
+// below runs instead wherever one call cannot reproduce it: a giant amount whose matrix is not direct, baby steps whose
+// prime sets or factors differ (so that addCtxt would rescale, or dropSmallAndSpecialPrimes would keep a set other than S),
+// a CKKS bad dimension, giant steps whose sum would not be a plain add (different intFactor or ratFactor), or no rotated
+// giant step at all.
+inline void MatMul1DBSGS(Ctxt& ctxt, long gen, long D, const std::vector<BsgsDiag>& cache, const std::vector<BsgsDiag>& cache1 = {}) {
+  using P = BasicAutomorphPrecon;
+  if (D <= 0 || (long)cache.size() != D || (!cache1.empty() && (long)cache1.size() != D)) throw InvalidArgument("MatMul1DBSGS: one diagonal per index");
+  const bool native = cache1.empty();
+  const Context& context = ctxt.context;
+  const KeyInfo& pubKey = ctxt.pubKey;
+  const long m = context.getM();
+  long g = (long)std::sqrt((double)D); while (g * g < D) g++; while (g > 1 && (g - 1) * (g - 1) >= D) g--;
+  const long h = (D + g - 1) / g;
+  std::vector<std::shared_ptr<Ctxt>> bs = GenBabySteps(ctxt, gen, g, native), bs1;
+  if (!native) { Ctxt c1(ctxt); c1.smartAutomorph(genToPow(gen, -D, m)); bs1 = GenBabySteps(c1, gen, g, false); }
+  auto mulAdd = [&](Ctxt& acc, const BsgsDiag& d, const Ctxt& b) { if (!d.c) return; Ctxt tmp(b); P::mulConst(tmp, d); acc += tmp; };
+  auto loop = [&]() {   // src/matmul.cpp:1022-1057 and 1097-1142, one partition
+    Ctxt acc(pubKey, ctxt.ptxtSpace);
+    for (long k = 0; k < h; k++) {
+      Ctxt inner(pubKey, ctxt.ptxtSpace);
+      for (long j = 0; j < g; j++) {
+        const long i = j + g * k;
+        if (i >= D) break;
+        mulAdd(inner, cache[(size_t)i], *bs[(size_t)j]);
+        if (!native) mulAdd(inner, cache1[(size_t)i], *bs1[(size_t)j]);
+      }
+      if (k > 0) inner.smartAutomorph(genToPow(gen, g * k, m));
+      acc += inner;
+    }
+    ctxt = acc;
+  };
+  auto meta_of = [&](const Ctxt& c) {
+    Ctxt t(pubKey, c.ptxtSpace);
+    t.primeSet = c.primeSet; t.noiseBound = c.noiseBound; t.intFactor = c.intFactor; t.ratFactor = c.ratFactor; t.ptxtMag = c.ptxtMag;
+    return t;
+  };
+  // ---- can one call reproduce the loop?
+  const bool ckks = ctxt.isCKKS();
+  const long keyID = ctxt.getKeyID();
+  const IndexSet special = context.getSpecialPrimes();
+  std::vector<const Ctxt*> all;
+  for (auto& b : bs) all.push_back(b.get());
+  for (auto& b : bs1) all.push_back(b.get());
+  const IndexSet S = bs[0]->primeSet;
+  bool ok = !(ckks && !native) && S <= context.getCtxtPrimes() && S.disjointFrom(context.getSmallPrimes()) && S.disjointFrom(special);
+  for (size_t a = 0; ok && a < all.size(); a++) {
+    const Ctxt& b = *all[a];
+    const bool j0 = a % (size_t)g == 0;
+    ok = b.parts.size() == 2 && b.getPartIndexByHandle(SKHandle()) >= 0 && b.getPartIndexByHandle(SKHandle(1, 1, keyID)) >= 0 &&
+         b.primeSet == (native || j0 ? S : (S | special)) && b.ptxtSpace == bs[0]->ptxtSpace && b.intFactor == bs[0]->intFactor;
+  }
+  std::vector<uint64_t> kg((size_t)h, 1), scal((size_t)h, 1);
+  std::vector<const KeySwitch*> W((size_t)h, nullptr);
+  std::vector<Ctxt> inner;   // metadata of each giant step's acc_inner; empty ones are skipped as addCtxt skips them
+  std::vector<char> nonempty((size_t)h, 0);
+  bool anyrot = false;
+  long nd = 0;   // the digits of S (src/DoubleCRT.cpp:485-493)
+  for (IndexSet rem = S; !empty(rem) && nd < (long)context.getDigits().size(); nd++) rem.remove(context.getDigit(nd));
+  for (long k = 0; ok && k < h; k++) {
+    Ctxt im(pubKey, ctxt.ptxtSpace);
+    bool first = true, high = false;
+    for (long j = 0; ok && j < g && j + g * k < D; j++)
+      for (int list = 0; list < (native ? 1 : 2); list++) {
+        const BsgsDiag& d = (list ? cache1 : cache)[(size_t)(j + g * k)];
+        if (!d.c) continue;
+        Ctxt t = meta_of(*(list ? bs1 : bs)[(size_t)j]);
+        P::mulConstMeta(t, d);
+        if (!first && ckks) { Ctxt x = meta_of(im); P::modUpMeta(x, t.primeSet); Ctxt y = t; P::modUpMeta(y, im.primeSet); if (x.ratFactor < y.ratFactor || y.ratFactor < x.ratFactor) ok = false; }
+        P::addMeta(im, first, t);
+        high = high || j > 0;
+      }
+    inner.push_back(im);
+    nonempty[(size_t)k] = !first;
+    if (first) continue;
+    if (!native && !high) ok = false;   // acc_inner over S alone would be relinearised as the native form's
+    const long kk = genToPow(gen, g * k, m);
+    if (k == 0 || kk == 1) continue;
+    if (!pubKey.isReachable(kk, keyID)) { ok = false; break; }
+    const KeySwitch* w = pubKey.getNextKSWmatrix(kk, keyID);
+    if (w->fromKey.powerOfX != kk || w->toKeyID != keyID || (long)w->b.size() < nd) { ok = false; break; }
+    kg[(size_t)k] = (uint64_t)kk; W[(size_t)k] = w; anyrot = true;
+    Ctxt x = im;
+    x.relin_CKKS_adjust();   // metadata only: the native form has no mod-down before it
+    if (ckks) { const XD r = x.ratFactor / im.ratFactor; scal[(size_t)k] = (uint64_t)std::llround(r.to_double()); }
+  }
+  if (!ok || !anyrot) { loop(); return; }
+  // ---- the call
+  const long nb = native ? g : 2 * g;
+  std::vector<DoubleCRT> up;   // the extended form's j = 0 baby steps, brought to S | special (addCtxt's scaling by P)
+  if (!native)
+    for (const Ctxt* b : {bs[0].get(), bs1[0].get()})
+      for (int pt = 0; pt < 2; pt++) { up.push_back(b->parts[(size_t)b->getPartIndexByHandle(pt ? SKHandle(1, 1, keyID) : SKHandle())].dcrt); up.back().addPrimesAndScale(special); }
+  std::vector<hb_poly*> b0, b1, cs((size_t)(h * nb), nullptr), ea((size_t)(h * nd), nullptr), eb((size_t)(h * nd), nullptr);
+  for (long a = 0; a < nb; a++) {
+    const Ctxt& b = *(a < g ? bs : bs1)[(size_t)(a % g)];
+    const long ui = a == 0 ? 0 : a == g ? 2 : -1;
+    b0.push_back(!native && ui >= 0 ? up[(size_t)ui].handle() : b.parts[(size_t)b.getPartIndexByHandle(SKHandle())].dcrt.handle());
+    b1.push_back(!native && ui >= 0 ? up[(size_t)ui + 1].handle() : b.parts[(size_t)b.getPartIndexByHandle(SKHandle(1, 1, keyID))].dcrt.handle());
+  }
+  for (long k = 0; k < h; k++) {
+    for (long j = 0; j < g && j + g * k < D; j++) {
+      if (cache[(size_t)(j + g * k)].c) cs[(size_t)(k * nb + j)] = cache[(size_t)(j + g * k)].c->handle();
+      if (!native && cache1[(size_t)(j + g * k)].c) cs[(size_t)(k * nb + g + j)] = cache1[(size_t)(j + g * k)].c->handle();
+    }
+    if (W[(size_t)k]) for (long i = 0; i < nd; i++) { ea[(size_t)(k * nd + i)] = W[(size_t)k]->aHandle((size_t)i); eb[(size_t)(k * nd + i)] = W[(size_t)k]->b[(size_t)i].handle(); }
+  }
+  const IndexSet full = S | special;
+  DoubleCRT a0(context, full), a1(context, full);
+  std::vector<double> norms((size_t)h * (kNormStride8 + 2), 0.0);
+  {
+    hb_poly* o0[1] = {a0.handle()}; hb_poly* o1[1] = {a1.handle()};
+    auto Sv = S.vec();
+    check(hb_bsgs_linear_map_norm(b0.data(), b1.data(), (int)nb, 1, Sv.data(), (int)Sv.size(), native ? 0 : 1, (uint64_t)bs[0]->ptxtSpace,
+                                  (int)h, kg.data(), cs.data(), scal.data(), ea.data(), eb.data(), (int)nd, o0, o1, 0, norms.data()));
+  }
+  // ---- metadata: the loop's, giant step by giant step in its order
+  Ctxt meta(pubKey, ctxt.ptxtSpace);
+  bool first = true;
+  const double logP = pubKey.logOfProduct(special);
+  for (long k = 0; k < h; k++) {
+    if (!nonempty[(size_t)k]) continue;
+    Ctxt t = inner[(size_t)k];
+    if (W[(size_t)k]) {   // smartAutomorph: automorph, reLinearize (dropSmallAndSpecialPrimes, relin_CKKS_adjust, keySwitchPart)
+      const double* nr = &norms[(size_t)k * (kNormStride8 + 2)];
+      if (!native) {      // modDownToSet(S): parts 1 and s, the noise of delta/P from the device
+        const XD addedNoise = XD(nr[kNormStride8]) + XD(nr[kNormStride8 + 1]) * XD::exp(std::log(pubKey.skBound));
+        const XD f = XD::exp(pubKey.logOfProduct(special));
+        t.ratFactor = t.ratFactor / f;
+        t.noiseBound = t.noiseBound / f;
+        t.noiseBound = t.noiseBound + addedNoise;
+        t.primeSet = S;
+      }
+      t.relin_CKKS_adjust();
+      Ctxt tmp(pubKey, t.ptxtSpace);
+      tmp.intFactor = t.intFactor; tmp.ptxtMag = t.ptxtMag;
+      tmp.noiseBound = t.noiseBound * XD::exp(logP);
+      tmp.primeSet = t.primeSet | special;
+      tmp.ratFactor = t.ratFactor * XD::exp(logP);
+      if (!ckks) tmp.reducePtxtSpace(W[(size_t)k]->ptxtSpace);
+      XD addedNoise(0.0);
+      for (long i = 0; i < nd; i++) addedNoise = addedNoise + XD::exp(nr[i]);
+      addedNoise = addedNoise * W[(size_t)k]->noiseBound;
+      tmp.noiseBound = tmp.noiseBound + addedNoise;
+      t = tmp;
+    }
+    if (!first) {   // acc += term must be a plain add
+      Ctxt x = meta, y = t;
+      P::modUpMeta(x, t.primeSet); P::modUpMeta(y, meta.primeSet);
+      if (x.ptxtSpace != y.ptxtSpace || x.intFactor != y.intFactor || (ckks && (x.ratFactor < y.ratFactor || y.ratFactor < x.ratFactor))) { loop(); return; }
+    }
+    P::addMeta(meta, first, t);
+  }
+  Ctxt out(pubKey, meta.ptxtSpace);
+  out.primeSet = meta.primeSet; out.noiseBound = meta.noiseBound; out.intFactor = meta.intFactor;
+  out.ratFactor = meta.ratFactor; out.ptxtMag = meta.ptxtMag;
+  out.parts.emplace_back(a0, SKHandle());
+  out.parts.emplace_back(a1, SKHandle(1, 1, keyID));
+  ctxt = out;
+}
 
 // ---- SURVEY 8f-2: the steps either side of the path ------------------------------------------------------------
 // Sampling follows the reference's DISTRIBUTIONS (src/sample.cpp); its bit stream (NTL's PRG) is not restated, so
