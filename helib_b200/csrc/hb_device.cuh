@@ -950,6 +950,74 @@ __global__ void __launch_bounds__(HB_THREADS) k_ks_giant(const HbPrimeDev* __res
   }
 }
 
+// Block linear map (BlockMatMul1DExec::mul's non-iterative branches, src/matmul.cpp:1782-1974), first pass: the hoisted
+// rotations BasicAutomorphPrecon::automorph(k_t) of a chunk of inner amounts, written for the items of a launch, i.e.
+// k_ks_linmap's inner loop without the constant:
+//   k_t != 1: out0 = scal*sigma_kt(c0) + sum_i sigma_kt(D_i)*b_{t,i},  out1 = sum_i sigma_kt(D_i)*a_{t,i}
+//   k_t == 1: out0 = scal*c0, out1 = scal*c1                      (addPrimesAndScale of the S ciphertext)
+// Each inner product (at most HB_MAXDIG + 1 products below 2^120) is summed in 128 bits and reduced once.  Amount t of
+// item it writes slot t*nitems + it.  grid = (coefficient blocks, rows, item groups of NI), as k_ks_linmap.
+#define HB_HOIST_MAXAMT 64      // inner amounts per launch
+#define HB_HOIST_SLOTS 128      // rotations x items in a chunk: the rotation scratch of hb_block_linear_map
+struct HbHoistJob {
+  u64 N, m;
+  const int* rep; const int* irep;   // general m; null: power-of-two m
+  int ndig, nitems, namt;
+  HbRows rows;
+  u64 scal[HB_MAXROWS];              // P mod q on the rows of S, 0 on the special rows
+  u64 k[HB_HOIST_MAXAMT];
+  const u64* evk_a[HB_HOIST_MAXAMT][HB_MAXDIG];
+  const u64* evk_b[HB_HOIST_MAXAMT][HB_MAXDIG];
+  const u64* dig[HB_MAXB][HB_MAXDIG];
+  const u64* c0[HB_MAXB];
+  const u64* c1[HB_MAXB];
+  u64* out0[HB_HOIST_SLOTS];
+  u64* out1[HB_HOIST_SLOTS];
+};
+template <int NI>
+__global__ void __launch_bounds__(HB_THREADS) k_ks_hoist(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT HbHoistJob J) {
+  const int pi = J.rows.prime[blockIdx.y];
+  const HbPrimeDev P = primes[pi];
+  const size_t N = (size_t)J.N;
+  const size_t off = (size_t)pi * N;
+  const u64 sc = J.scal[blockIdx.y];
+  const int it0 = blockIdx.z * NI;
+  const int cnt = J.nitems - it0 < NI ? J.nitems - it0 : NI;
+  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < N; j += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = off + j;
+    const u64 rj = J.rep ? (u64)J.rep[j] : 2 * (u64)j + 1;   // m <= 2^20: rj*k < 2^41
+    for (int t = 0; t < J.namt; t++) {
+      const u64 k = J.k[t];
+      const int s0 = t * J.nitems + it0;
+      if (k == 1) {
+#pragma unroll
+        for (int u = 0; u < NI; u++)
+          if (u < cnt) {
+            J.out0[s0 + u][o] = hb_mulmod(J.c0[it0 + u][o], sc, P);
+            J.out1[s0 + u][o] = hb_mulmod(J.c1[it0 + u][o], sc, P);
+          }
+        continue;
+      }
+      const size_t g = off + (J.rep ? (size_t)J.irep[(rj * k) % J.m] : (size_t)(((rj * k) & (J.m - 1)) >> 1));
+      u64 p0h[NI], p0l[NI], p1h[NI], p1l[NI];
+#pragma unroll
+      for (int u = 0; u < NI; u++) {
+        p0h[u] = 0; p0l[u] = 0; p1h[u] = 0; p1l[u] = 0;
+        if (sc && u < cnt) hb_mac128(p0h[u], p0l[u], J.c0[it0 + u][g], sc);
+      }
+      for (int i = 0; i < J.ndig; i++) {
+        const u64 b = J.evk_b[t][i][o], a = J.evk_a[t][i][o];
+#pragma unroll
+        for (int u = 0; u < NI; u++)
+          if (u < cnt) { const u64 d = J.dig[it0 + u][i][g]; hb_mac128(p0h[u], p0l[u], d, b); hb_mac128(p1h[u], p1l[u], d, a); }
+      }
+#pragma unroll
+      for (int u = 0; u < NI; u++)
+        if (u < cnt) { J.out0[s0 + u][o] = hb_reduce128(p0h[u], p0l[u], P); J.out1[s0 + u][o] = hb_reduce128(p1h[u], p1l[u], P); }
+    }
+  }
+}
+
 
 // ------------------------------------------------------------------------------------------
 // Canonical-embedding norm (noise metadata): max_j |f(zeta^(2j+1))|, zeta = e^(i*pi/N), in FP64.

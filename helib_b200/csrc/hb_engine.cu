@@ -121,6 +121,7 @@ struct hb_ctx {
   int prg_window = 0;   // HB_PRG_WINDOW=w: count w buffers per row in parallel instead of the statistical bound (tests the slow path)
   std::vector<hb_poly*> ks_a;   // a_i regenerated from a seeded evk_a for the key switch in flight (allocated on first use)
   std::vector<hb_poly*> bsgs;   // hb_bsgs_linear_map: rotated sums and their digits, HB_BSGS_GROUP*(2+ndig) polys (first use)
+  std::vector<hb_poly*> block;  // hb_block_linear_map: rotations, rotated sums, digits and set-1 sums (first use)
 };
 // The row schedule of a seeded set (hb_poly_create_seeded): the ChaCha20 key, the rows, and in one device allocation the
 // first buffer of every schedule row (start[T+1]) and the exclusive row offset of every counted buffer (off[T*wmax]).
@@ -349,6 +350,7 @@ extern "C" void hb_ctx_destroy(hb_ctx* c) {
   cudaFree(c->prg_start); cudaFree(c->prg_off); cudaFree(c->prg_ticket);
   for (hb_poly* p : c->ks_a) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->bsgs) { cudaFree(p->d); delete p; }
+  for (hb_poly* p : c->block) { cudaFree(p->d); delete p; }
   for (HbTmap* sl : c->tmap_slabs) cudaFree(sl);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
   delete c;
@@ -2339,6 +2341,152 @@ extern "C" int hb_bsgs_linear_map_norm(hb_poly* const* baby0, hb_poly* const* ba
   return bsgs_impl(baby0, baby1, nbaby, nitems, S, nS, extended, ptxt_space, ngiant, kgiant, consts, scal, evk_a, evk_b, ndig_evk,
                    acc0, acc1, accumulate, norms);
 }
+// Terms per k_ks_giant launch: the 128-bit budget, and with seeded keys the key scratch (HB_LINMAP_SEEDED polys)
+static int bsgs_tmax(int nd, bool seeded) {
+  return std::max(1, std::min(254 / (nd + 1), seeded ? HB_LINMAP_SEEDED / std::max(1, nd) : HB_BSGS_GROUP));
+}
+// BSGS step 1 over one group of nit items (of at most ic): slot a*nit + it of X0/X1 (+)= sigma_{k_a}( scal[a] * sum_b cst(a, b) * baby(it, b) ) over the rows
+// R, for a < ng, it < nit, b < nbaby.  cst(a, b) is the constant (null: a zero diagonal) and baby(it, b) the two parts of a
+// baby step; kinv[a] = k_a^-1 mod m; accumulate adds to the sums already in the slots.  One k_bsgs_mac pass per NI items,
+// NT terms, nbl baby steps and HB_MAXROWS rows.
+template <class CstF, class BabyF>
+static int bsgs_mac(hb_ctx* c, const std::vector<int32_t>& R, hb_poly* const* X0, hb_poly* const* X1, int ic, int nit, int ng, int nbaby,
+                    const u64* kinv, const uint64_t* scal, bool accumulate, CstF cst, BabyF baby) {
+  const int nR = (int)R.size();
+  const int NI = ic >= 4 ? 4 : ic >= 2 ? 2 : 1, NT = HB_BSGS_MACW / NI;
+  const int nbl = std::min(HB_BSGS_MAXBABY, std::min(HB_BSGS_CST / NT, HB_BSGS_BABY / NI));   // baby steps per k_bsgs_mac launch
+  for (int u0 = 0; u0 < nit; u0 += NI) {
+    const int ni = std::min(NI, nit - u0);
+    for (int a0 = 0; a0 < ng; a0 += NT) {
+      const int nt = std::min(NT, ng - a0);
+      for (int b0 = 0; b0 < nbaby; b0 += nbl) {
+        const int nb = std::min(nbl, nbaby - b0);
+        const bool add = accumulate || b0 > 0;
+        for (int r0 = 0; r0 < nR; r0 += HB_MAXROWS) {
+          const int nr = std::min(HB_MAXROWS, nR - r0);
+          HbBsgsMacJob J; memset(&J, 0, sizeof(J));
+          J.N = c->N; J.m = c->m;
+          if (c->gen.on) { J.rep = c->gen.d_rep; J.irep = c->gen.d_irep; }
+          J.nb = nb; J.nt = nt; J.ni = ni; J.accumulate = add;
+          fill_rows(J.rows, R.data() + r0, nr);
+          u64 ncst = 0;
+          for (int a = 0; a < nt; a++) {
+            J.kinv[a] = kinv[a0 + a]; J.scal[a] = scal ? scal[a0 + a] : 1;
+            for (int b = 0; b < nb; b++) {
+              hb_poly* cp = cst(a0 + a, b0 + b);
+              J.cst[a * nb + b] = cp ? cp->d : nullptr;
+              ncst += cp != nullptr;
+            }
+            for (int u = 0; u < ni; u++) {
+              const int s = (a0 + a) * nit + u0 + u;
+              J.out0[a * NI + u] = X0[s]->d; J.out1[a * NI + u] = X1[s]->d;
+            }
+          }
+          for (int u = 0; u < ni; u++)
+            for (int b = 0; b < nb; b++) {
+              const std::pair<hb_poly*, hb_poly*> x = baby(u0 + u, b0 + b);
+              J.baby0[u * nb + b] = x.first->d; J.baby1[u * nb + b] = x.second->d;
+            }
+          const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, 1);
+          pre_launch(c);
+          switch (NI) {
+            case 1: HB_LAUNCH(k_bsgs_mac<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+            case 2: HB_LAUNCH(k_bsgs_mac<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+            default: HB_LAUNCH(k_bsgs_mac<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+          }
+          // the baby rows of the items and the constant rows of the giant steps once; two sums written per pair
+          // (and read when a later baby chunk adds to them)
+          HB_TRY(post_launch(c, "k_bsgs_mac", ((u64)2 * ni * nb + ncst + (u64)(add ? 4 : 2) * ni * nt) * nr * c->N * 8));
+        }
+      }
+    }
+  }
+  return HB_OK;
+}
+// BSGS steps 2-3 over one group of ng terms of nit items, slot a*nit + it of X0/X1 holding term a's rotated sum (digits in
+// DG[slot*nd ..]): for kt[a] != 1 the mod-down to S (extended form) and breakIntoDigits, batched over the group, then the key
+// switch with matrix a (evk_a/evk_b + a*ndig_evk) and the unrotated terms, summed into acc0/acc1[it], tmax terms and at most
+// HB_BSGS_GROUP slots per k_ks_giant launch.  acc_on: the accumulators hold a sum (becomes true).  norms (optional): term a
+// of item it at norms + (it*nstride + a)*(HB_MAXDIG + 2), as hb_bsgs_linear_map_norm lays them out.
+static int bsgs_finish(hb_ctx* c, hb_poly* const* X0, hb_poly* const* X1, hb_poly* const* DG, int nit, int ng, const uint64_t* kt,
+                       hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk, int nd, const int32_t* S, int nS,
+                       const std::vector<int32_t>& Sp, int extended, uint64_t ptxt_space, const std::vector<u64>& scp,
+                       const std::vector<u64>& scx, int tmax, bool seeded, hb_poly* const* acc0, hb_poly* const* acc1, bool& acc_on,
+                       double* norms, size_t nstride) {
+  const int nSp = (int)Sp.size();
+  tmax = std::max(1, std::min(tmax, HB_BSGS_GROUP / nit));
+  std::vector<hb_poly*> rot0, rot01, rdig, list, ka;
+  // 2. the rotated sums' mod-down (extended form) and digits, batched over the group
+  for (int a = 0; a < ng; a++) {
+    if (kt[a] == 1) continue;
+    for (int it = 0; it < nit; it++) {
+      const int s = a * nit + it;
+      rot0.push_back(X1[s]); rot01.push_back(X0[s]); rot01.push_back(X1[s]);
+      for (int i = 0; i < nd; i++) rdig.push_back(DG[(size_t)s * nd + i]);
+    }
+  }
+  if (!rot0.empty()) {
+    std::vector<double> sdn(norms && extended ? rot01.size() : 0), ldn(norms ? rdig.size() : 0);
+    if (extended) HB_TRY(scale_down_impl(rot01.data(), (int)rot01.size(), Sp.data(), nSp, S, nS, ptxt_space, norms ? sdn.data() : nullptr));
+    int ndo = 0;
+    HB_TRY(break_into_digits_impl(rot0.data(), (int)rot0.size(), S, nS, rdig.data(), nd, &ndo, norms ? ldn.data() : nullptr));
+    for (int a = 0, r = 0; norms && a < ng; a++) {
+      if (kt[a] == 1) continue;
+      for (int it = 0; it < nit; it++, r++) {
+        double* o = norms + ((size_t)it * nstride + a) * (HB_MAXDIG + 2);
+        for (int i = 0; i < nd; i++) o[i] = ldn[(size_t)r * nd + i];
+        if (extended) { o[HB_MAXDIG] = sdn[(size_t)2 * r]; o[HB_MAXDIG + 1] = sdn[(size_t)2 * r + 1]; }
+      }
+    }
+  }
+  // 3. key switch and sum, tmax terms per launch
+  for (int a0 = 0; a0 < ng;) {
+    int nt = 0, nrot = 0;
+    while (a0 + nt < ng && nt < tmax) { nrot += kt[a0 + nt] != 1; nt++; if (seeded && (nrot + 1) * nd > HB_LINMAP_SEEDED) break; }
+    list.clear();
+    for (int a = 0; a < nt; a++) {
+      const int t = a0 + a;
+      if (kt[t] != 1) list.insert(list.end(), evk_a + (size_t)t * ndig_evk, evk_a + (size_t)t * ndig_evk + nd);
+    }
+    if (!list.empty()) HB_TRY(ks_expand_a(c, list.data(), (int)list.size(), Sp.data(), nSp, ka));
+    u64 item_rows = 0, key_rows = 0;   // rows read per item and shared by the items, per row of the launch
+    for (int r0 = 0; r0 < nSp; r0 += HB_MAXROWS) {
+      const int nr = std::min(HB_MAXROWS, nSp - r0);
+      HbGiantJob J; memset(&J, 0, sizeof(J));
+      J.N = c->N; J.ndig = nd; J.nitems = nit; J.nt = nt; J.accumulate = acc_on ? 1 : 0;
+      fill_rows(J.rows, Sp.data() + r0, nr);
+      for (int i = 0; i < nr; i++) { J.scp[i] = scp[(size_t)(r0 + i)]; J.scx[i] = scx[(size_t)(r0 + i)]; }
+      item_rows = 0; key_rows = 0;
+      for (int a = 0, slot = 0; a < nt; a++) {
+        const int t = a0 + a;
+        J.plain[a] = kt[t] == 1;
+        if (!J.plain[a]) {
+          for (int i = 0; i < nd; i++) { J.evk_a[a][i] = ka[(size_t)slot * nd + i]->d; J.evk_b[a][i] = evk_b[(size_t)t * ndig_evk + i]->d; }
+          slot++;
+        }
+        item_rows += J.plain[a] ? 2 : nd + 1; key_rows += J.plain[a] ? 0 : 2 * nd;
+        for (int it = 0; it < nit; it++) {
+          const int s = (a0 + a) * nit + it, sl = a * nit + it;
+          J.x0[sl] = X0[s]->d; J.x1[sl] = X1[s]->d;
+          for (int i = 0; i < nd && !J.plain[a]; i++) J.dig[sl][i] = DG[(size_t)s * nd + i]->d;
+        }
+      }
+      for (int it = 0; it < nit; it++) { J.acc0[it] = acc0[it]->d; J.acc1[it] = acc1[it]->d; }
+      const int ni = nit >= 4 ? 4 : nit >= 2 ? 2 : 1;
+      const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, (unsigned)((nit + ni - 1) / ni));
+      pre_launch(c);
+      switch (ni) {
+        case 1: HB_LAUNCH(k_ks_giant<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+        case 2: HB_LAUNCH(k_ks_giant<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+        default: HB_LAUNCH(k_ks_giant<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+      }
+      HB_TRY(post_launch(c, "k_ks_giant", ((item_rows + (acc_on ? 4 : 2)) * nit + key_rows) * nr * c->N * 8));
+    }
+    acc_on = true;
+    a0 += nt;
+  }
+  return HB_OK;
+}
 static int bsgs_impl(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, int nitems, const int32_t* S, int nS, int extended,
                      uint64_t ptxt_space, int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
                      hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk, hb_poly* const* acc0, hb_poly* const* acc1,
@@ -2408,7 +2556,6 @@ static int bsgs_impl(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, in
   std::vector<u64> kinv((size_t)ngiant);
   for (int t = 0; t < ngiant; t++) h_invmod(kgiant[t], c->m, &kinv[(size_t)t]);
   const std::vector<int32_t> R = extended ? Sp : std::vector<int32_t>(S, S + nS);   // the rows of the baby steps
-  const int nR = (int)R.size();
   // scratch: slot s of a group holds the rotated sum (x0, x1) of one (giant step, item) and its nd digits
   const int G = std::min(HB_BSGS_GROUP, nitems * ngiant);   // a group never holds more pairs than the call has
   while ((int)c->bsgs.size() < G * (2 + nd)) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->bsgs.push_back(p); }
@@ -2417,135 +2564,240 @@ static int bsgs_impl(hb_poly* const* baby0, hb_poly* const* baby1, int nbaby, in
   hb_poly* const* DG = X0 + 2 * G;
   const int ic = std::min(nitems, G);                 // items per group
   const int gg = std::max(1, G / ic);                 // giant steps per group
-  const int NI = ic >= 4 ? 4 : ic >= 2 ? 2 : 1, NT = HB_BSGS_MACW / NI;
-  const int nbl = std::min(HB_BSGS_MAXBABY, std::min(HB_BSGS_CST / NT, HB_BSGS_BABY / NI));   // baby steps per k_bsgs_mac launch
-  // terms per k_ks_giant launch: the 128-bit budget, and with seeded keys the key scratch (HB_LINMAP_SEEDED polys)
-  const int tmax = std::max(1, std::min(254 / (nd + 1), seeded ? HB_LINMAP_SEEDED / std::max(1, nd) : G));
+  const int tmax = bsgs_tmax(nd, seeded);
   bool acc_on = accumulate != 0;
-  std::vector<hb_poly*> rot0, rot01, rdig, list, ka;
   for (int i0 = 0; i0 < nitems; i0 += ic) {
     const int nit = std::min(ic, nitems - i0);
     acc_on = accumulate != 0;
     for (int t0 = 0; t0 < ngiant; t0 += gg) {
       const int ng = std::min(gg, ngiant - t0);
       // 1. the rotated inner sums of the group: slot a*nit + it
-      for (int u0 = 0; u0 < nit; u0 += NI) {
-        const int ni = std::min(NI, nit - u0);
-        for (int a0 = 0; a0 < ng; a0 += NT) {
-          const int nt = std::min(NT, ng - a0);
-          for (int b0 = 0; b0 < nbaby; b0 += nbl) {
-            const int nb = std::min(nbl, nbaby - b0);
-            for (int r0 = 0; r0 < nR; r0 += HB_MAXROWS) {
-              const int nr = std::min(HB_MAXROWS, nR - r0);
-              HbBsgsMacJob J; memset(&J, 0, sizeof(J));
-              J.N = c->N; J.m = c->m;
-              if (c->gen.on) { J.rep = c->gen.d_rep; J.irep = c->gen.d_irep; }
-              J.nb = nb; J.nt = nt; J.ni = ni; J.accumulate = b0 > 0;
-              fill_rows(J.rows, R.data() + r0, nr);
-              u64 ncst = 0;
-              for (int a = 0; a < nt; a++) {
-                const int t = t0 + a0 + a;
-                J.kinv[a] = kinv[(size_t)t]; J.scal[a] = scal ? scal[t] : 1;
-                for (int b = 0; b < nb; b++) {
-                  hb_poly* cp = consts[(size_t)t * nbaby + b0 + b];
-                  J.cst[a * nb + b] = cp ? cp->d : nullptr;
-                  ncst += cp != nullptr;
-                }
-                for (int u = 0; u < ni; u++) {
-                  const int s = (a0 + a) * nit + u0 + u;
-                  J.out0[a * NI + u] = X0[s]->d; J.out1[a * NI + u] = X1[s]->d;
-                }
-              }
-              for (int u = 0; u < ni; u++)
-                for (int b = 0; b < nb; b++) {
-                  const size_t e = (size_t)(i0 + u0 + u) * nbaby + b0 + b;
-                  J.baby0[u * nb + b] = baby0[e]->d; J.baby1[u * nb + b] = baby1[e]->d;
-                }
-              const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, 1);
-              pre_launch(c);
-              switch (NI) {
-                case 1: HB_LAUNCH(k_bsgs_mac<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
-                case 2: HB_LAUNCH(k_bsgs_mac<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
-                default: HB_LAUNCH(k_bsgs_mac<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
-              }
-              // the baby rows of the items and the constant rows of the giant steps once; two sums written per pair
-              // (and read when a later baby chunk adds to them)
-              HB_TRY(post_launch(c, "k_bsgs_mac", ((u64)2 * ni * nb + ncst + (u64)(b0 > 0 ? 4 : 2) * ni * nt) * nr * c->N * 8));
-            }
-          }
-        }
+      HB_TRY(bsgs_mac(c, R, X0, X1, ic, nit, ng, nbaby, kinv.data() + t0, scal ? scal + t0 : nullptr, false,
+                      [&](int a, int b) { return consts[(size_t)(t0 + a) * nbaby + b]; },
+                      [&](int u, int b) { const size_t e = (size_t)(i0 + u) * nbaby + b; return std::make_pair(baby0[e], baby1[e]); }));
+      // 2-3. their mod-down (extended form), digits and key switch, summed into the accumulators
+      HB_TRY(bsgs_finish(c, X0, X1, DG, nit, ng, kgiant + t0, evk_a + (size_t)t0 * ndig_evk, evk_b + (size_t)t0 * ndig_evk, ndig_evk, nd,
+                         S, nS, Sp, extended, ptxt_space, scp, scx, tmax, seeded, acc0 + i0, acc1 + i0, acc_on,
+                         norms ? norms + ((size_t)i0 * ngiant + t0) * (HB_MAXDIG + 2) : nullptr, (size_t)ngiant));
+    }
+  }
+  return HB_OK;
+}
+
+// Block linear map (SURVEY 8f-1): BlockMatMul1DExec::mul's non-iterative branches with one interval (src/matmul.cpp:1782-1868
+// native, 1869-1974 bad dimension).  Output o < n1*(bad ? 2 : 1) is set o / n1's sum for outer amount k1[o % n1].  Per item
+// chunk and per group of outputs: k_ks_hoist writes the hoisted rotations of a chunk of at most HB_HOIST_SLOTS / items
+// inner amounts, k_bsgs_mac folds them into the group's rotated sums (the rotations play the baby steps, the outer amounts
+// the giant steps), and bsgs_finish mod-downs, key-switches and sums them -- the set-0 sums into the accumulators, the set-1
+// sums into a scratch sum that is finally rotated by kfinal and added.  When all inner amounts fit one chunk, the rotations
+// are formed once per item chunk; otherwise once per chunk and group.
+#define HB_BLOCK_GROUP 64       // outputs x items per group
+extern "C" int hb_automorph(hb_poly* const* dst, hb_poly* const* src, int nitems, const int32_t* idx, int n, uint64_t k);
+static int block_impl(hb_poly* const* digits, int maxdig, int nitems, const int32_t* S, int nS, hb_poly* const* c0, hb_poly* const* c1,
+                      uint64_t ptxt_space, int n0, const uint64_t* k0, hb_poly* const* evk0_a, hb_poly* const* evk0_b,
+                      int n1, const uint64_t* k1, hb_poly* const* evk1_a, hb_poly* const* evk1_b,
+                      hb_poly* const* consts, hb_poly* const* consts1, uint64_t kfinal, hb_poly* const* evkf_a, hb_poly* const* evkf_b,
+                      int ndig_evk, hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms);
+extern "C" int hb_block_linear_map(hb_poly* const* digits, int maxdig, int nitems, const int32_t* S, int nS,
+                                   hb_poly* const* c0, hb_poly* const* c1, uint64_t ptxt_space,
+                                   int n0, const uint64_t* k0, hb_poly* const* evk0_a, hb_poly* const* evk0_b,
+                                   int n1, const uint64_t* k1, hb_poly* const* evk1_a, hb_poly* const* evk1_b,
+                                   hb_poly* const* consts, hb_poly* const* consts1, uint64_t kfinal,
+                                   hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                                   hb_poly* const* acc0, hb_poly* const* acc1, int accumulate) {
+  return block_impl(digits, maxdig, nitems, S, nS, c0, c1, ptxt_space, n0, k0, evk0_a, evk0_b, n1, k1, evk1_a, evk1_b, consts, consts1,
+                    kfinal, evkf_a, evkf_b, ndig_evk, acc0, acc1, accumulate, nullptr);
+}
+extern "C" int hb_block_linear_map_norm(hb_poly* const* digits, int maxdig, int nitems, const int32_t* S, int nS,
+                                        hb_poly* const* c0, hb_poly* const* c1, uint64_t ptxt_space,
+                                        int n0, const uint64_t* k0, hb_poly* const* evk0_a, hb_poly* const* evk0_b,
+                                        int n1, const uint64_t* k1, hb_poly* const* evk1_a, hb_poly* const* evk1_b,
+                                        hb_poly* const* consts, hb_poly* const* consts1, uint64_t kfinal,
+                                        hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                                        hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms) {
+  if (!norms) return hb_fail(HB_ERR_BAD_ARG, "hb_block_linear_map_norm: null output");
+  return block_impl(digits, maxdig, nitems, S, nS, c0, c1, ptxt_space, n0, k0, evk0_a, evk0_b, n1, k1, evk1_a, evk1_b, consts, consts1,
+                    kfinal, evkf_a, evkf_b, ndig_evk, acc0, acc1, accumulate, norms);
+}
+static int block_impl(hb_poly* const* digits, int maxdig, int nitems, const int32_t* S, int nS, hb_poly* const* c0, hb_poly* const* c1,
+                      uint64_t ptxt_space, int n0, const uint64_t* k0, hb_poly* const* evk0_a, hb_poly* const* evk0_b,
+                      int n1, const uint64_t* k1, hb_poly* const* evk1_a, hb_poly* const* evk1_b,
+                      hb_poly* const* consts, hb_poly* const* consts1, uint64_t kfinal, hb_poly* const* evkf_a, hb_poly* const* evkf_b,
+                      int ndig_evk, hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms) {
+  static const char* who = "hb_block_linear_map";
+  hb_ctx* c = nullptr;
+  const bool bad = consts1 != nullptr;
+  if (n0 <= 0 || n1 <= 0 || nitems <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: n0, n1 and nitems must be positive", who);
+  if (!k0 || !k1 || !consts) return hb_fail(HB_ERR_BAD_ARG, "%s: no amounts", who);
+  HB_TRY(check_polys(c0, nitems, &c, "hb_block_linear_map(c0)"));
+  HB_TRY(check_polys(c1, nitems, &c, "hb_block_linear_map(c1)"));
+  HB_TRY(check_idx(c, S, nS, who));
+  if (ptxt_space < 1) return hb_fail(HB_ERR_BAD_ARG, "%s: ptxt_space must be at least 1", who);
+  if (c->special.empty()) return hb_fail(HB_ERR_BAD_ARG, "%s: context has no special primes", who);
+  for (int i = 0; i < nS; i++) if (c->digit_of[S[i]] < 0) return hb_fail(HB_ERR_INDEX_SET, "%s: S must be a subset of the ctxt primes (prime %d)", who, S[i]);
+  auto unit = [&](uint64_t k) { return k != 0 && k < c->m && h_gcd((long)k, (long)c->m) == 1; };
+  bool anyk = bad && kfinal != 1;
+  for (int t = 0; t < n0; t++) { if (!unit(k0[t])) return hb_fail(HB_ERR_INDEX_SET, "automorph: k not in Zm*"); anyk |= k0[t] != 1; }
+  for (int t = 0; t < n1; t++) { if (!unit(k1[t])) return hb_fail(HB_ERR_INDEX_SET, "automorph: k not in Zm*"); anyk |= k1[t] != 1; }
+  if (bad && !unit(kfinal)) return hb_fail(HB_ERR_INDEX_SET, "automorph: k not in Zm*");
+  for (int i = 0; i < n0 * n1; i++) if (consts[i]) HB_TRY(check_polys(consts + i, 1, &c, "hb_block_linear_map(consts)"));
+  for (int i = 0; bad && i < n0 * n1; i++) if (consts1[i]) HB_TRY(check_polys(consts1 + i, 1, &c, "hb_block_linear_map(consts1)"));
+  HB_TRY(check_polys(acc0, nitems, &c, "hb_block_linear_map(acc0)")); HB_TRY(check_polys(acc1, nitems, &c, "hb_block_linear_map(acc1)"));
+  int nd = 0;   // the digits of S (src/DoubleCRT.cpp:485-493)
+  {
+    std::vector<char> rem(c->nprimes, 0); int left = nS;
+    for (int i = 0; i < nS; i++) rem[S[i]] = 1;
+    for (; left > 0; nd++) for (int i = 0; i < c->nprimes; i++) if (rem[i] && c->digit_of[i] == nd) { rem[i] = 0; left--; }
+  }
+  if (nd > maxdig) return hb_fail(HB_ERR_BAD_ARG, "%s: S has %d digits, maxdig is %d", who, nd, maxdig);
+  HB_TRY(check_polys(digits, nitems * maxdig, &c, "hb_block_linear_map(digits)"));
+  // matrix t of a set of amounts: entries t*ndig_evk .. t*ndig_evk + nd
+  struct Keys { int n; const uint64_t* k; hb_poly* const* a; hb_poly* const* b; const char* name; };
+  const Keys sets[3] = {{n0, k0, evk0_a, evk0_b, "evk0"}, {n1, k1, evk1_a, evk1_b, "evk1"}, {bad ? 1 : 0, &kfinal, evkf_a, evkf_b, "evkf"}};
+  if (anyk && (nd > ndig_evk || nd > HB_MAXDIG)) return hb_fail(HB_ERR_BAD_ARG, "%s: key-switching matrices have %d columns, need %d", who, ndig_evk, nd);
+  for (const Keys& K : sets)
+    for (int t = 0; t < K.n; t++) {
+      if (K.k[t] == 1) continue;
+      if (!K.a || !K.b) return hb_fail(HB_ERR_BAD_ARG, "%s: no key-switching matrices (%s)", who, K.name);
+      HB_TRY(check_polys(K.a + (size_t)t * ndig_evk, nd, &c, "hb_block_linear_map(evk_a)", true));
+      HB_TRY(check_polys(K.b + (size_t)t * ndig_evk, nd, &c, "hb_block_linear_map(evk_b)"));
+    }
+  // the accumulators are written while every other operand is still being read: they must be distinct and alias nothing
+  std::set<const hb_poly*> in, out;
+  in.insert(c0, c0 + nitems); in.insert(c1, c1 + nitems); in.insert(digits, digits + (size_t)nitems * maxdig);
+  for (int i = 0; i < n0 * n1; i++) { if (consts[i]) in.insert(consts[i]); if (bad && consts1[i]) in.insert(consts1[i]); }
+  for (const Keys& K : sets)
+    for (int t = 0; t < K.n; t++)
+      if (K.k[t] != 1) { in.insert(K.a + (size_t)t * ndig_evk, K.a + (size_t)t * ndig_evk + nd); in.insert(K.b + (size_t)t * ndig_evk, K.b + (size_t)t * ndig_evk + nd); }
+  out.insert(acc0, acc0 + nitems); out.insert(acc1, acc1 + nitems);
+  if ((int)out.size() != 2 * nitems) return hb_fail(HB_ERR_BAD_ARG, "%s: the accumulators must be distinct polynomials", who);
+  for (const hb_poly* p : out) if (in.count(p)) return hb_fail(HB_ERR_BAD_ARG, "%s: an accumulator aliases an input", who);
+  std::vector<int32_t> Sp(S, S + nS); Sp.insert(Sp.end(), c->special.begin(), c->special.end()); std::sort(Sp.begin(), Sp.end());
+  const int nSp = (int)Sp.size();
+  bool seeded = false;
+  for (const Keys& K : sets)
+    for (int t = 0; t < K.n; t++)
+      for (int i = 0; K.k[t] != 1 && i < nd; i++) {
+        const HbSeedSched* Q = K.a[(size_t)t * ndig_evk + i]->sched;
+        if (!Q) continue;
+        seeded = true;
+        for (int32_t r : Sp) if (!std::binary_search(Q->idx.begin(), Q->idx.end(), r)) return hb_fail(HB_ERR_INDEX_SET, "%s: row %d is not in the seeded set", who, r);
       }
-      // 2. the rotated sums' mod-down (extended form) and digits, batched over the group
-      rot0.clear(); rot01.clear(); rdig.clear();
-      for (int a = 0; a < ng; a++) {
-        if (kgiant[t0 + a] == 1) continue;
+  // ---- every argument is checked: nothing was launched before this point
+  std::vector<u64> scp((size_t)nSp, 0), scx((size_t)nSp, 1);   // the rotated sums are over S | special: extended form
+  for (int r = 0; r < nSp; r++)
+    if (std::find(S, S + nS, Sp[r]) != S + nS) scp[(size_t)r] = prod_mod(c, c->special.data(), (int)c->special.size(), c->q[Sp[r]]);
+  const int nout = bad ? 2 * n1 : n1;
+  const int T = nout + (bad ? 1 : 0);                  // norm entries per item
+  std::vector<u64> kinv((size_t)nout);
+  std::vector<uint64_t> kout((size_t)nout);
+  for (int o = 0; o < nout; o++) { kout[(size_t)o] = k1[o % n1]; h_invmod(kout[(size_t)o], c->m, &kinv[(size_t)o]); }
+  // scratch: H*ic rotations (both parts), G rotated sums with their digits, and the set-1 sum of every item of a chunk
+  const int G = std::min(HB_BLOCK_GROUP, nitems * nout);
+  const int ic = std::min(std::min(nitems, G), HB_BSGS_GROUP);   // items per chunk (k_ks_giant takes at most HB_BSGS_GROUP)
+  const int gg = std::max(1, G / ic);                              // outputs per group
+  const int H = std::min(n0, HB_HOIST_SLOTS / ic);                 // inner amounts per chunk
+  const int nslot = H * ic;
+  const size_t need = (size_t)2 * nslot + (size_t)G * (2 + nd) + (bad ? 2 * ic : 0);
+  while (c->block.size() < need) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->block.push_back(p); }
+  hb_poly* const* ROT0 = c->block.data();
+  hb_poly* const* ROT1 = ROT0 + nslot;
+  hb_poly* const* X0 = ROT1 + nslot;
+  hb_poly* const* X1 = X0 + G;
+  hb_poly* const* DG = X1 + G;
+  hb_poly* const* Y0 = DG + (size_t)G * nd;             // the set-1 sums
+  hb_poly* const* Y1 = Y0 + ic;
+  const int tmax = bsgs_tmax(nd, seeded);
+  const int achunk = seeded ? std::max(1, HB_LINMAP_SEEDED / nd) : HB_HOIST_MAXAMT;   // inner amounts per k_ks_hoist launch
+  std::vector<hb_poly*> list, ka;
+  std::vector<int> slot;
+  // the rotations of inner amounts h0 .. h0+hc of items i0 .. i0+nit: amount b of item it into slot b*nit + it
+  auto hoist = [&](int i0, int nit, int h0, int hc) -> int {
+    for (int a0 = 0; a0 < hc; a0 += achunk) {
+      const int na = std::min(achunk, hc - a0);
+      list.clear(); slot.assign((size_t)na, -1);
+      for (int a = 0; a < na; a++) {
+        const int t = h0 + a0 + a;
+        if (k0[t] != 1) { slot[(size_t)a] = (int)list.size(); list.insert(list.end(), evk0_a + (size_t)t * ndig_evk, evk0_a + (size_t)t * ndig_evk + nd); }
+      }
+      if (!list.empty()) HB_TRY(ks_expand_a(c, list.data(), (int)list.size(), Sp.data(), nSp, ka));
+      u64 item_rows = 0, key_rows = 0;   // rows read and written per item, and read once, per row of the launch
+      for (int a = 0; a < na; a++) { item_rows += k0[h0 + a0 + a] == 1 ? 4 : nd + 3; key_rows += k0[h0 + a0 + a] == 1 ? 0 : 2 * nd; }
+      for (int r0 = 0; r0 < nSp; r0 += HB_MAXROWS) {
+        const int nr = std::min(HB_MAXROWS, nSp - r0);
+        HbHoistJob J; memset(&J, 0, sizeof(J));
+        J.N = c->N; J.m = c->m;
+        if (c->gen.on) { J.rep = c->gen.d_rep; J.irep = c->gen.d_irep; }
+        J.ndig = nd; J.nitems = nit; J.namt = na;
+        fill_rows(J.rows, Sp.data() + r0, nr);
+        for (int i = 0; i < nr; i++) J.scal[i] = scp[(size_t)(r0 + i)];
+        for (int a = 0; a < na; a++) {
+          const int t = h0 + a0 + a;
+          J.k[a] = k0[t];
+          if (slot[(size_t)a] >= 0)
+            for (int i = 0; i < nd; i++) { J.evk_a[a][i] = ka[(size_t)slot[(size_t)a] + i]->d; J.evk_b[a][i] = evk0_b[(size_t)t * ndig_evk + i]->d; }
+          for (int it = 0; it < nit; it++) { J.out0[a * nit + it] = ROT0[(a0 + a) * nit + it]->d; J.out1[a * nit + it] = ROT1[(a0 + a) * nit + it]->d; }
+        }
         for (int it = 0; it < nit; it++) {
-          const int s = a * nit + it;
-          rot0.push_back(X1[s]); rot01.push_back(X0[s]); rot01.push_back(X1[s]);
-          for (int i = 0; i < nd; i++) rdig.push_back(DG[(size_t)s * nd + i]);
+          J.c0[it] = c0[i0 + it]->d; J.c1[it] = c1[i0 + it]->d;
+          for (int i = 0; i < nd; i++) J.dig[it][i] = digits[(size_t)(i0 + it) * maxdig + i]->d;
         }
-      }
-      if (!rot0.empty()) {
-        std::vector<double> sdn(norms && extended ? rot01.size() : 0), ldn(norms ? rdig.size() : 0);
-        if (extended) HB_TRY(scale_down_impl(rot01.data(), (int)rot01.size(), Sp.data(), nSp, S, nS, ptxt_space, norms ? sdn.data() : nullptr));
-        int ndo = 0;
-        HB_TRY(break_into_digits_impl(rot0.data(), (int)rot0.size(), S, nS, rdig.data(), nd, &ndo, norms ? ldn.data() : nullptr));
-        for (int a = 0, r = 0; norms && a < ng; a++) {
-          if (kgiant[t0 + a] == 1) continue;
-          for (int it = 0; it < nit; it++, r++) {
-            double* o = norms + ((size_t)(i0 + it) * ngiant + t0 + a) * (HB_MAXDIG + 2);
-            for (int i = 0; i < nd; i++) o[i] = ldn[(size_t)r * nd + i];
-            if (extended) { o[HB_MAXDIG] = sdn[(size_t)2 * r]; o[HB_MAXDIG + 1] = sdn[(size_t)2 * r + 1]; }
-          }
+        const int ni = nit >= 4 ? 4 : nit >= 2 ? 2 : 1;
+        const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, (unsigned)((nit + ni - 1) / ni));
+        pre_launch(c);
+        switch (ni) {
+          case 1: HB_LAUNCH(k_ks_hoist<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+          case 2: HB_LAUNCH(k_ks_hoist<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
+          default: HB_LAUNCH(k_ks_hoist<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
         }
-      }
-      // 3. key switch and sum, tmax terms per launch
-      for (int a0 = 0; a0 < ng;) {
-        int nt = 0, nrot = 0;
-        while (a0 + nt < ng && nt < tmax) { nrot += kgiant[t0 + a0 + nt] != 1; nt++; if (seeded && (nrot + 1) * nd > HB_LINMAP_SEEDED) break; }
-        list.clear();
-        for (int a = 0; a < nt; a++) {
-          const int t = t0 + a0 + a;
-          if (kgiant[t] != 1) list.insert(list.end(), evk_a + (size_t)t * ndig_evk, evk_a + (size_t)t * ndig_evk + nd);
-        }
-        if (!list.empty()) HB_TRY(ks_expand_a(c, list.data(), (int)list.size(), Sp.data(), nSp, ka));
-        u64 item_rows = 0, key_rows = 0;   // rows read per item and shared by the items, per row of the launch
-        for (int r0 = 0; r0 < nSp; r0 += HB_MAXROWS) {
-          const int nr = std::min(HB_MAXROWS, nSp - r0);
-          HbGiantJob J; memset(&J, 0, sizeof(J));
-          J.N = c->N; J.ndig = nd; J.nitems = nit; J.nt = nt; J.accumulate = acc_on ? 1 : 0;
-          fill_rows(J.rows, Sp.data() + r0, nr);
-          for (int i = 0; i < nr; i++) { J.scp[i] = scp[(size_t)(r0 + i)]; J.scx[i] = scx[(size_t)(r0 + i)]; }
-          item_rows = 0; key_rows = 0;
-          for (int a = 0, slot = 0; a < nt; a++) {
-            const int t = t0 + a0 + a;
-            J.plain[a] = kgiant[t] == 1;
-            if (!J.plain[a]) {
-              for (int i = 0; i < nd; i++) { J.evk_a[a][i] = ka[(size_t)slot * nd + i]->d; J.evk_b[a][i] = evk_b[(size_t)t * ndig_evk + i]->d; }
-              slot++;
-            }
-            item_rows += J.plain[a] ? 2 : nd + 1; key_rows += J.plain[a] ? 0 : 2 * nd;
-            for (int it = 0; it < nit; it++) {
-              const int s = (a0 + a) * nit + it, sl = a * nit + it;
-              J.x0[sl] = X0[s]->d; J.x1[sl] = X1[s]->d;
-              for (int i = 0; i < nd && !J.plain[a]; i++) J.dig[sl][i] = DG[(size_t)s * nd + i]->d;
-            }
-          }
-          for (int it = 0; it < nit; it++) { J.acc0[it] = acc0[i0 + it]->d; J.acc1[it] = acc1[i0 + it]->d; }
-          const int ni = nit >= 4 ? 4 : nit >= 2 ? 2 : 1;
-          const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, (unsigned)((nit + ni - 1) / ni));
-          pre_launch(c);
-          switch (ni) {
-            case 1: HB_LAUNCH(k_ks_giant<1>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
-            case 2: HB_LAUNCH(k_ks_giant<2>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
-            default: HB_LAUNCH(k_ks_giant<4>, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J); break;
-          }
-          HB_TRY(post_launch(c, "k_ks_giant", ((item_rows + (acc_on ? 4 : 2)) * nit + key_rows) * nr * c->N * 8));
-        }
-        acc_on = true;
-        a0 += nt;
+        HB_TRY(post_launch(c, "k_ks_hoist", (item_rows * nit + key_rows) * nr * c->N * 8));
       }
     }
+    return HB_OK;
+  };
+  const bool once = n0 <= H;
+  for (int i0 = 0; i0 < nitems; i0 += ic) {
+    const int nit = std::min(ic, nitems - i0);
+    bool acc_on = accumulate != 0, y_on = false;
+    if (once) HB_TRY(hoist(i0, nit, 0, n0));
+    for (int o0 = 0; o0 < nout; o0 += gg) {
+      const int ng = std::min(gg, nout - o0);
+      // 1. the group's rotated sums sigma_k1( sum_i consts[i*n1 + j] * r_i ): slot a*nit + it
+      for (int h0 = 0; h0 < n0; h0 += H) {
+        const int hc = std::min(H, n0 - h0);
+        if (!once) HB_TRY(hoist(i0, nit, h0, hc));
+        HB_TRY(bsgs_mac(c, Sp, X0, X1, ic, nit, ng, hc, kinv.data() + o0, nullptr, h0 > 0,
+                        [&](int a, int b) { const int o = o0 + a; return (o < n1 ? consts : consts1)[(size_t)(h0 + b) * n1 + o % n1]; },
+                        [&](int u, int b) { return std::make_pair(ROT0[b * nit + u], ROT1[b * nit + u]); }));
+      }
+      // 2-3. set 0 into the accumulators, set 1 into its sum
+      const int split = std::max(0, std::min(ng, n1 - o0));
+      double* nb = norms ? norms + ((size_t)i0 * T + o0) * (HB_MAXDIG + 2) : nullptr;
+      if (split > 0)
+        HB_TRY(bsgs_finish(c, X0, X1, DG, nit, split, kout.data() + o0, evk1_a + (size_t)o0 * ndig_evk, evk1_b + (size_t)o0 * ndig_evk, ndig_evk,
+                           nd, S, nS, Sp, 1, ptxt_space, scp, scx, tmax, seeded, acc0 + i0, acc1 + i0, acc_on, nb, (size_t)T));
+      if (ng > split) {
+        const int j0 = o0 + split - n1;
+        HB_TRY(bsgs_finish(c, X0 + (size_t)split * nit, X1 + (size_t)split * nit, DG + (size_t)split * nit * nd, nit, ng - split, k1 + j0,
+                           evk1_a + (size_t)j0 * ndig_evk, evk1_b + (size_t)j0 * ndig_evk, ndig_evk, nd, S, nS, Sp, 1, ptxt_space, scp, scx,
+                           tmax, seeded, Y0, Y1, y_on, nb ? nb + (size_t)split * (HB_MAXDIG + 2) : nullptr, (size_t)T));
+      }
+    }
+    if (!bad) continue;
+    // the bad dimension's last term: the set-1 sum rotated by kfinal (smartAutomorph), added to the accumulators
+    double* nf = norms ? norms + ((size_t)i0 * T + nout) * (HB_MAXDIG + 2) : nullptr;
+    if (kfinal == 1) {
+      HB_TRY(bsgs_finish(c, Y0, Y1, DG, nit, 1, &kfinal, evkf_a, evkf_b, ndig_evk, nd, S, nS, Sp, 1, ptxt_space, scp, scx, tmax, seeded,
+                         acc0 + i0, acc1 + i0, acc_on, nf, (size_t)T));
+      continue;
+    }
+    // sigma_kfinal as a gather copy into the group slots: one read and one write of the set-1 sums, once per item chunk.
+    // Folding it into a k_bsgs_mac pass would need a constant row of ones to multiply by, which reads as much; the
+    // checks of hb_automorph cannot fail here (its operands are this call's scratch, kfinal was checked above).
+    HB_TRY(hb_automorph(X0, Y0, nit, Sp.data(), nSp, kfinal));
+    HB_TRY(hb_automorph(X1, Y1, nit, Sp.data(), nSp, kfinal));
+    HB_TRY(bsgs_finish(c, X0, X1, DG, nit, 1, &kfinal, evkf_a, evkf_b, ndig_evk, nd, S, nS, Sp, 1, ptxt_space, scp, scx, tmax, seeded,
+                       acc0 + i0, acc1 + i0, acc_on, nf, (size_t)T));
   }
   return HB_OK;
 }

@@ -580,9 +580,49 @@ def _engine_hoist(cls):
                                              sc.ctypes.data_as(u64p) if sc is not None else None, keys(evk_a), keys(evk_b), nd,
                                              _arr(acc0), _arr(acc1), int(bool(accumulate))))
 
+    def block_linear_map(self, digits, S, c0, c1, k0, evk0_a, evk0_b, k1, evk1_a, evk1_b, consts, acc0, acc1,
+                         consts1=None, kfinal=1, evkf_a=None, evkf_b=None, ptxt_space=1, accumulate=False, norms=False):
+        """acc (+)= BlockMatMul1DExec's non-iterative branches over S | special, for every item (hb_block_linear_map).
+        digits: per item, the digit Polys of c1; consts / consts1: per inner amount, one Poly (or None) per outer amount;
+        consts1 (with kfinal and its matrix evkf_a / evkf_b) selects the bad dimension; evk*_a / evk*_b: per amount, the list
+        of matrix Polys (None where the amount is 1).  norms=True calls hb_block_linear_map_norm and returns its norms as
+        [item][entry][10] (entry j: set 0's term j; n1 + j: set 1's; 2*n1: the final term; NaN where not written)."""
+        a, p, n = _idx(S)
+        nd = len(digits[0])
+        n0, n1 = len(k0), len(k1)
+
+        def amounts(ks):
+            return np.ascontiguousarray(np.array([int(x) for x in ks], dtype=np.uint64))
+
+        def blocks(cs):
+            return (C.c_void_p * (n0 * n1))(*[c_.h if c_ is not None else None for row in cs for c_ in row])
+
+        def keys(evk, cnt):
+            arr = (C.c_void_p * max(1, cnt * nd))()
+            for j, mat in enumerate(evk):
+                for i in range(nd):
+                    arr[j * nd + i] = mat[i].h if mat is not None else None
+            return arr
+        kk0, kk1 = amounts(k0), amounts(k1)
+        bad = consts1 is not None
+        args = (_arr([d for item in digits for d in item]), nd, len(digits), p, n, _arr(c0), _arr(c1),
+                C.c_uint64(int(ptxt_space)), n0, kk0.ctypes.data_as(u64p), keys(evk0_a, n0), keys(evk0_b, n0),
+                n1, kk1.ctypes.data_as(u64p), keys(evk1_a, n1), keys(evk1_b, n1), blocks(consts),
+                blocks(consts1) if bad else None, C.c_uint64(int(kfinal)),
+                keys([evkf_a], 1) if bad else None, keys([evkf_b], 1) if bad else None, nd,
+                _arr(acc0), _arr(acc1), int(bool(accumulate)))
+        if not norms:
+            self._ck(self.lib.hb_block_linear_map(*args))
+            return None
+        T = 2 * n1 + 1 if bad else n1
+        out = np.full((len(digits), T, 10), np.nan, dtype=np.float64)
+        self._ck(self.lib.hb_block_linear_map_norm(*args, out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
+
     cls.automorph_keyswitch_digits = automorph_keyswitch_digits
     cls.hoisted_linear_map = hoisted_linear_map
     cls.bsgs_linear_map = bsgs_linear_map
+    cls.block_linear_map = block_linear_map
     return cls
 
 

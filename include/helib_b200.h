@@ -253,6 +253,48 @@ int hb_bsgs_linear_map_norm(hb_poly* const* baby0, hb_poly* const* baby1, int nb
                             int ngiant, const uint64_t* kgiant, hb_poly* const* consts, const uint64_t* scal,
                             hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk,
                             hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms);
+/* Block linear map (SURVEY 8f-1): BlockMatMul1DExec::mul's non-iterative branches with one PartitionInfo interval
+ * (src/matmul.cpp:1782-1868 native, 1869-1974 bad dimension), i.e. a GF(p)-linear map on slots of degree d.  digits =
+ * hb_break_into_digits of c1 over S ([item*maxdig + i], maxdig at least the digits of S); c0, c1 over S.  Inner amounts
+ * k0[i] (i < n0) with matrices evk0 (s(X^k0) -> s), outer amounts k1[j] (j < n1) with matrices evk1; consts[i*n1 + j] over
+ * S | special (HElib's cache.multiplier[i*d1 + j]; NULL: a zero block, skipped as MulAdd skips it).  consts1 != NULL
+ * selects the bad dimension: consts1 has the layout of consts, kfinal is genToPow(dim, -D) with matrix evkf.  For every
+ * item, over S | special, in HElib's order of steps:
+ *   r_i = BasicAutomorphPrecon::automorph(k0[i])   (k0[i] == 1: P*(c0, c1), addPrimesAndScale)
+ *   a_j = sum_i consts[i*n1 + j] * r_i,  a1_j likewise with consts1
+ *   term(x, k) = x for k == 1; otherwise smartAutomorph(k) in the extended form of hb_bsgs_linear_map: sigma_k, the mod-down
+ *     to S (scaleDownToSet with ptxt_space), breakIntoDigits over S and the key switch
+ *   acc0/acc1 (+)= sum_j term(a_j, k1[j])  [ + term( sum_j term(a1_j, k1[j]), kfinal ) ]      (accumulate = 0 overwrites)
+ * evk*_a/evk*_b hold ndig_evk entries per matrix (matrix t = entries t*ndig_evk ..; evkf one matrix), ignored and may be
+ * NULL where the amount is 1; they need as many columns as S has digits.  The items share everything but digits, c0, c1,
+ * acc0 and acc1.  Power-of-two and general m; expanded or seeded evk_a.  Per chunk of items (at most 32) and group of
+ * outputs ((j, set) pairs, at most 64 with the items): k_ks_hoist writes the rotations of at most 128/items inner amounts,
+ * k_bsgs_mac folds them into the group's rotated sums, and the mod-down, digits and k_ks_giant follow as in
+ * hb_bsgs_linear_map.  The scratch is at most 2*min(128, n0*ic) + min(64, nitems*n1*(bad ? 2 : 1))*(2 + ndig) + (bad ?
+ * 2*ic : 0) polys, ic = min(32, nitems): it does not grow with n0 past 128/ic inner amounts, nor with n1.  Errors, all
+ * reported before any launch: an amount not in Z_m^*, S not within the ctxt primes, or a seeded evk_a without a needed row
+ * -> HB_ERR_INDEX_SET; n0, n1 or nitems <= 0, no amounts, too few digit slots or matrix columns, a missing matrix, an
+ * accumulator aliasing an input or another accumulator, or a seeded handle other than in evk_a -> HB_ERR_BAD_ARG.
+ * Stream-ordered, no synchronisation; after the first call, a call of the same shape allocates nothing. */
+int hb_block_linear_map(hb_poly* const* digits, int maxdig, int nitems, const int32_t* S, int nS,
+                        hb_poly* const* c0, hb_poly* const* c1, uint64_t ptxt_space,
+                        int n0, const uint64_t* k0, hb_poly* const* evk0_a, hb_poly* const* evk0_b,
+                        int n1, const uint64_t* k1, hb_poly* const* evk1_a, hb_poly* const* evk1_b,
+                        hb_poly* const* consts, hb_poly* const* consts1, uint64_t kfinal,
+                        hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                        hb_poly* const* acc0, hb_poly* const* acc1, int accumulate);
+/* The same, returning the norms the noise bookkeeping of smartAutomorph needs for every rotated term, in the layout of
+ * hb_bsgs_linear_map_norm: with T = n1 (native) or 2*n1 + 1 (bad dimension), norms[(item*T + e)*(8 + 2) + i] = ln ||E_i||
+ * of digit i (i < ndig), and at offsets 8 and 9 the ||delta/P|| of parts 0 and 1 of the mod-down.  Entry e = j is term
+ * (a_j, k1[j]); in the bad dimension e = n1 + j is term (a1_j, k1[j]) and e = 2*n1 the final term (kfinal).  Entries of
+ * unrotated terms are not written.  Synchronises (host values). */
+int hb_block_linear_map_norm(hb_poly* const* digits, int maxdig, int nitems, const int32_t* S, int nS,
+                             hb_poly* const* c0, hb_poly* const* c1, uint64_t ptxt_space,
+                             int n0, const uint64_t* k0, hb_poly* const* evk0_a, hb_poly* const* evk0_b,
+                             int n1, const uint64_t* k1, hb_poly* const* evk1_a, hb_poly* const* evk1_b,
+                             hb_poly* const* consts, hb_poly* const* consts1, uint64_t kfinal,
+                             hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                             hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms);
 /* Ctxt::tensorProduct of two canonical 2-part ciphertexts (src/Ctxt.cpp:1563-1608) */
 int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1,
               hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int nitems, const int32_t* idx, int n);

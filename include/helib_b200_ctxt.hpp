@@ -766,6 +766,11 @@ class BasicAutomorphPrecon {
   std::vector<DoubleCRT> polyDigits;
  public:
   double lastKSNoiseRatioHoist = 0;   // "KS-noise-ratio-hoist" (src/matmul.cpp:101)
+  // the cleaned ciphertext, the noise bound of every hoisted rotation and the digits of its part 1 (hb::BlockMatMul1D
+  // hands them to one engine call)
+  const Ctxt& cleaned() const { return ctxt; }
+  const XD& hoistNoise() const { return noise; }
+  const std::vector<DoubleCRT>& digits() const { return polyDigits; }
   explicit BasicAutomorphPrecon(const Ctxt& c) : ctxt(c), noise(1.0) {
     if (ctxt.parts.size() >= 1 && !ctxt.parts[0].skHandle.isOne()) throw LogicError("Invalid ciphertext (secret key handle for part 0 is not one)");
     if (ctxt.parts.size() <= 1) return;
@@ -990,6 +995,34 @@ inline std::vector<std::shared_ptr<Ctxt>> GenBabySteps(const Ctxt& ctxt, long ge
 using BsgsDiag = BasicAutomorphPrecon::Coef;
 // hb_bsgs_linear_map_norm: per giant step, 8 digit log-norms then the two mod-down norms
 constexpr long kNormStride8 = 8;
+// The metadata smartAutomorph gives a rotated term with a direct matrix W, replayed from the norms the device returned
+// (nr: nd digit log-norms, then at kNormStride8 the two mod-down norms): if extended (over S | special), modDownToSet(S);
+// then relin_CKKS_adjust and keySwitchPart.
+inline void relinTermMeta(Ctxt& t, const double* nr, bool extended, const KeySwitch& W, long nd, const IndexSet& S) {
+  const KeyInfo& pubKey = t.pubKey;
+  const IndexSet special = t.context.getSpecialPrimes();
+  const double logP = pubKey.logOfProduct(special);
+  if (extended) {      // modDownToSet(S): parts 1 and s, the noise of delta/P from the device
+    const XD addedNoise = XD(nr[kNormStride8]) + XD(nr[kNormStride8 + 1]) * XD::exp(std::log(pubKey.skBound));
+    const XD f = XD::exp(logP);
+    t.ratFactor = t.ratFactor / f;
+    t.noiseBound = t.noiseBound / f;
+    t.noiseBound = t.noiseBound + addedNoise;
+    t.primeSet = S;
+  }
+  t.relin_CKKS_adjust();
+  Ctxt tmp(pubKey, t.ptxtSpace);
+  tmp.intFactor = t.intFactor; tmp.ptxtMag = t.ptxtMag;
+  tmp.noiseBound = t.noiseBound * XD::exp(logP);
+  tmp.primeSet = t.primeSet | special;
+  tmp.ratFactor = t.ratFactor * XD::exp(logP);
+  if (!t.isCKKS()) tmp.reducePtxtSpace(W.ptxtSpace);
+  XD addedNoise(0.0);
+  for (long i = 0; i < nd; i++) addedNoise = addedNoise + XD::exp(nr[i]);
+  addedNoise = addedNoise * W.noiseBound;
+  tmp.noiseBound = tmp.noiseBound + addedNoise;
+  t = tmp;
+}
 // MatMul1DExec::mul for a dimension of size D > HELIB_KEYSWITCH_THRESH with generator gen, not iterative: ctxt becomes
 // sum_i cache[i] * rot_i(ctxt) (+ cache1[i] * rot_{i-D}(ctxt) for a bad dimension, cache1 non-empty).  g = KSGiantStepSize(D).
 // The baby steps are built as GenBabySteps builds them; every giant step is then summed by one hb_bsgs_linear_map call,
@@ -1112,33 +1145,10 @@ inline void MatMul1DBSGS(Ctxt& ctxt, long gen, long D, const std::vector<BsgsDia
   // ---- metadata: the loop's, giant step by giant step in its order
   Ctxt meta(pubKey, ctxt.ptxtSpace);
   bool first = true;
-  const double logP = pubKey.logOfProduct(special);
   for (long k = 0; k < h; k++) {
     if (!nonempty[(size_t)k]) continue;
     Ctxt t = inner[(size_t)k];
-    if (W[(size_t)k]) {   // smartAutomorph: automorph, reLinearize (dropSmallAndSpecialPrimes, relin_CKKS_adjust, keySwitchPart)
-      const double* nr = &norms[(size_t)k * (kNormStride8 + 2)];
-      if (!native) {      // modDownToSet(S): parts 1 and s, the noise of delta/P from the device
-        const XD addedNoise = XD(nr[kNormStride8]) + XD(nr[kNormStride8 + 1]) * XD::exp(std::log(pubKey.skBound));
-        const XD f = XD::exp(pubKey.logOfProduct(special));
-        t.ratFactor = t.ratFactor / f;
-        t.noiseBound = t.noiseBound / f;
-        t.noiseBound = t.noiseBound + addedNoise;
-        t.primeSet = S;
-      }
-      t.relin_CKKS_adjust();
-      Ctxt tmp(pubKey, t.ptxtSpace);
-      tmp.intFactor = t.intFactor; tmp.ptxtMag = t.ptxtMag;
-      tmp.noiseBound = t.noiseBound * XD::exp(logP);
-      tmp.primeSet = t.primeSet | special;
-      tmp.ratFactor = t.ratFactor * XD::exp(logP);
-      if (!ckks) tmp.reducePtxtSpace(W[(size_t)k]->ptxtSpace);
-      XD addedNoise(0.0);
-      for (long i = 0; i < nd; i++) addedNoise = addedNoise + XD::exp(nr[i]);
-      addedNoise = addedNoise * W[(size_t)k]->noiseBound;
-      tmp.noiseBound = tmp.noiseBound + addedNoise;
-      t = tmp;
-    }
+    if (W[(size_t)k]) relinTermMeta(t, &norms[(size_t)k * (kNormStride8 + 2)], !native, *W[(size_t)k], nd, S);
     if (!first) {   // acc += term must be a plain add
       Ctxt x = meta, y = t;
       P::modUpMeta(x, t.primeSet); P::modUpMeta(y, meta.primeSet);
@@ -1146,6 +1156,172 @@ inline void MatMul1DBSGS(Ctxt& ctxt, long gen, long D, const std::vector<BsgsDia
     }
     P::addMeta(meta, first, t);
   }
+  Ctxt out(pubKey, meta.ptxtSpace);
+  out.primeSet = meta.primeSet; out.noiseBound = meta.noiseBound; out.intFactor = meta.intFactor;
+  out.ratFactor = meta.ratFactor; out.ptxtMag = meta.ptxtMag;
+  out.parts.emplace_back(a0, SKHandle());
+  out.parts.emplace_back(a1, SKHandle(1, 1, keyID));
+  ctxt = out;
+}
+
+// ---- BlockMatMul1DExec::mul's non-iterative branches (src/matmul.cpp:1663-1976) ------------------------------------
+// A GF(p)-linear map on slots of degree d along a dimension of size D with generator gen, both dimensions' strategy FULL
+// and one thread (one PartitionInfo interval): ctxt becomes sum_j sigma_{k1_j}( sum_i cache[i*d1 + j] * rot_{k0_i}(ctxt) )
+// (+ the same sum over cache1, rotated by gen^-D, for a bad dimension: cache1 non-empty).  Strategy +1 (D >= d) hoists
+// k0_i = gen^i, i < D, and rotates by the Frobenius k1_j = p^j, j < d; strategy -1 the other way round.  The map runs as one
+// hb_block_linear_map_norm call, with the loop's bits and its metadata (noise, factors, prime set) replayed term by term
+// from the norms the call returns.  The transcribed loop runs instead wherever one call cannot reproduce it: a ciphertext
+// that is not 2-part canonical after cleanUp, an amount whose matrix is not direct, an outer sum that is not over
+// S | special (so smartAutomorph would not mod down), sums that would not be a plain add, or no term at all.  The
+// iterative (HELIB_KSS_MIN) branches are not taken.  BGV only: HElib has no CKKS block executor.
+inline void BlockMatMul1D(Ctxt& ctxt, long gen, long D, long d, const std::vector<BsgsDiag>& cache, const std::vector<BsgsDiag>& cache1 = {}) {
+  using P = BasicAutomorphPrecon;
+  if (ctxt.isCKKS()) throw LogicError("BlockMatMul1DExec: not implemented for CKKS");
+  if (D <= 0 || d <= 0 || (long)cache.size() != D * d || (!cache1.empty() && (long)cache1.size() != D * d))
+    throw InvalidArgument("BlockMatMul1D: one block per (i, j)");
+  const bool bad = !cache1.empty();
+  const Context& context = ctxt.context;
+  const KeyInfo& pubKey = ctxt.pubKey;
+  const long m = context.getM();
+  const long p = context.getP();
+  const bool plus = D >= d;
+  const long d0 = plus ? D : d, d1 = plus ? d : D;
+  std::vector<long> k0((size_t)d0), k1((size_t)d1);
+  for (long i = 0; i < d0; i++) k0[(size_t)i] = plus ? genToPow(gen, i, m) : genToPow(p, i, m);
+  for (long j = 0; j < d1; j++) k1[(size_t)j] = plus ? genToPow(p, j, m) : genToPow(gen, j, m);
+  const long kf = genToPow(gen, -D, m);
+  ctxt.cleanUp();
+  auto mulAdd = [&](Ctxt& acc, const BsgsDiag& c, const Ctxt& r) { if (!c.c) return; Ctxt tmp(r); P::mulConst(tmp, c); acc += tmp; };
+  auto loop = [&]() {   // src/matmul.cpp:1782-1868 and 1869-1974, FULL strategies, one thread
+    BasicAutomorphPrecon precon(ctxt);
+    std::vector<Ctxt> acc((size_t)d1, Ctxt(pubKey, ctxt.ptxtSpace)), acc1(bad ? (size_t)d1 : 0, Ctxt(pubKey, ctxt.ptxtSpace));
+    for (long i = 0; i < d0; i++) {
+      std::shared_ptr<Ctxt> r = precon.automorph(k0[(size_t)i]);
+      for (long j = 0; j < d1; j++) {
+        mulAdd(acc[(size_t)j], cache[(size_t)(i * d1 + j)], *r);
+        if (bad) mulAdd(acc1[(size_t)j], cache1[(size_t)(i * d1 + j)], *r);
+      }
+    }
+    Ctxt sum(pubKey, ctxt.ptxtSpace), sum1(pubKey, ctxt.ptxtSpace);
+    for (long j = 0; j < d1; j++) {
+      if (j > 0) { acc[(size_t)j].smartAutomorph(k1[(size_t)j]); if (bad) acc1[(size_t)j].smartAutomorph(k1[(size_t)j]); }
+      sum += acc[(size_t)j];
+      if (bad) sum1 += acc1[(size_t)j];
+    }
+    if (bad) { sum1.smartAutomorph(kf); sum += sum1; }
+    ctxt = sum;
+  };
+  // ---- can one call reproduce the loop?
+  const long keyID = ctxt.getKeyID();
+  const IndexSet special = context.getSpecialPrimes();
+  const IndexSet S = ctxt.primeSet;
+  const IndexSet full = S | special;
+  bool ok = ctxt.parts.size() == 2 && ctxt.getPartIndexByHandle(SKHandle()) >= 0 && ctxt.getPartIndexByHandle(SKHandle(1, 1, keyID)) >= 0 &&
+            S <= context.getCtxtPrimes() && S.disjointFrom(context.getSmallPrimes()) && S.disjointFrom(special);
+  if (!ok) { loop(); return; }
+  long nd = 0;   // the digits of S (src/DoubleCRT.cpp:485-493)
+  for (IndexSet rem = S; !empty(rem) && nd < (long)context.getDigits().size(); nd++) rem.remove(context.getDigit(nd));
+  auto direct = [&](long k) -> const KeySwitch* {
+    if (k == 1) return nullptr;
+    if (!pubKey.isReachable(k, keyID)) { ok = false; return nullptr; }
+    const KeySwitch* w = pubKey.getNextKSWmatrix(k, keyID);
+    if (w->fromKey.powerOfX != k || w->toKeyID != keyID || (long)w->b.size() < nd) ok = false;
+    return w;
+  };
+  std::vector<const KeySwitch*> W0((size_t)d0), W1((size_t)d1);
+  for (long i = 0; i < d0; i++) W0[(size_t)i] = direct(k0[(size_t)i]);
+  for (long j = 1; j < d1; j++) W1[(size_t)j] = direct(k1[(size_t)j]);
+  const KeySwitch* Wf = bad ? direct(kf) : nullptr;
+  if (!ok) { loop(); return; }
+  BasicAutomorphPrecon precon(ctxt);
+  const Ctxt& cl = precon.cleaned();
+  auto meta_of = [&](const Ctxt& c) {
+    Ctxt t(pubKey, c.ptxtSpace);
+    t.primeSet = c.primeSet; t.noiseBound = c.noiseBound; t.intFactor = c.intFactor; t.ratFactor = c.ratFactor; t.ptxtMag = c.ptxtMag;
+    return t;
+  };
+  auto rot_meta = [&](long i) {   // BasicAutomorphPrecon::automorph(k0_i), metadata only
+    if (k0[(size_t)i] == 1) return meta_of(cl);
+    Ctxt t(pubKey, cl.ptxtSpace);
+    t.noiseBound = precon.hoistNoise(); t.intFactor = cl.intFactor; t.primeSet = full;
+    return t;
+  };
+  // the outer sums' metadata before their smartAutomorph: set 1 at n1 + j
+  const int nsets = bad ? 2 : 1;
+  std::vector<Ctxt> outer;
+  std::vector<char> nonempty;
+  bool any = false;
+  for (int set = 0; set < nsets; set++)
+    for (long j = 0; j < d1; j++) {
+      Ctxt a(pubKey, cl.ptxtSpace);
+      bool first = true;
+      for (long i = 0; i < d0; i++) {
+        const BsgsDiag& c = (set ? cache1 : cache)[(size_t)(i * d1 + j)];
+        if (!c.c) continue;
+        Ctxt t = rot_meta(i);
+        P::mulConstMeta(t, c);
+        P::addMeta(a, first, t);
+      }
+      outer.push_back(a); nonempty.push_back(!first);
+      any = any || !first;
+      if (!first && j > 0 && k1[(size_t)j] != 1 && !(a.primeSet == full)) ok = false;
+    }
+  if (!ok || !any) { loop(); return; }
+  // ---- the call
+  std::vector<hb_poly*> dg, cs((size_t)(d0 * d1), nullptr), cs1(bad ? (size_t)(d0 * d1) : 0, nullptr);
+  std::vector<hb_poly*> e0a((size_t)(d0 * nd), nullptr), e0b((size_t)(d0 * nd), nullptr), e1a((size_t)(d1 * nd), nullptr), e1b((size_t)(d1 * nd), nullptr);
+  std::vector<hb_poly*> efa((size_t)nd, nullptr), efb((size_t)nd, nullptr);
+  for (const DoubleCRT& x : precon.digits()) dg.push_back(x.handle());
+  for (long i = 0; i < d0 * d1; i++) {
+    if (cache[(size_t)i].c) cs[(size_t)i] = cache[(size_t)i].c->handle();
+    if (bad && cache1[(size_t)i].c) cs1[(size_t)i] = cache1[(size_t)i].c->handle();
+  }
+  auto keys = [&](const KeySwitch* w, hb_poly** a, hb_poly** b) { if (w) for (long i = 0; i < nd; i++) { a[i] = w->aHandle((size_t)i); b[i] = w->b[(size_t)i].handle(); } };
+  for (long i = 0; i < d0; i++) keys(W0[(size_t)i], &e0a[(size_t)(i * nd)], &e0b[(size_t)(i * nd)]);
+  for (long j = 0; j < d1; j++) keys(W1[(size_t)j], &e1a[(size_t)(j * nd)], &e1b[(size_t)(j * nd)]);
+  keys(Wf, efa.data(), efb.data());
+  std::vector<uint64_t> u0(k0.begin(), k0.end()), u1(k1.begin(), k1.end());
+  const long T = bad ? 2 * d1 + 1 : d1;
+  std::vector<double> norms((size_t)T * (kNormStride8 + 2), 0.0);
+  DoubleCRT a0(context, full), a1(context, full);
+  {
+    hb_poly* c0[1] = {cl.parts[(size_t)cl.getPartIndexByHandle(SKHandle())].dcrt.handle()};
+    hb_poly* c1[1] = {cl.parts[(size_t)cl.getPartIndexByHandle(SKHandle(1, 1, keyID))].dcrt.handle()};
+    hb_poly* o0[1] = {a0.handle()}; hb_poly* o1[1] = {a1.handle()};
+    auto Sv = S.vec();
+    check(hb_block_linear_map_norm(dg.data(), (int)dg.size(), 1, Sv.data(), (int)Sv.size(), c0, c1, (uint64_t)cl.ptxtSpace,
+                                   (int)d0, u0.data(), e0a.data(), e0b.data(), (int)d1, u1.data(), e1a.data(), e1b.data(),
+                                   cs.data(), bad ? cs1.data() : nullptr, (uint64_t)kf, efa.data(), efb.data(), (int)nd, o0, o1, 0, norms.data()));
+  }
+  // ---- metadata: the loop's, term by term in its order
+  auto plain = [&](const Ctxt& a, const Ctxt& b) {   // a += b must be a plain add
+    Ctxt x = a, y = b;
+    P::modUpMeta(x, b.primeSet); P::modUpMeta(y, a.primeSet);
+    return x.ptxtSpace == y.ptxtSpace && x.intFactor == y.intFactor;
+  };
+  Ctxt sums[2] = {Ctxt(pubKey, cl.ptxtSpace), Ctxt(pubKey, cl.ptxtSpace)};
+  bool firsts[2] = {true, true};
+  for (int set = 0; set < nsets; set++)
+    for (long j = 0; j < d1; j++) {
+      const size_t e = (size_t)(set * d1 + j);
+      if (!nonempty[e]) continue;
+      Ctxt t = outer[e];
+      if (j > 0 && W1[(size_t)j]) relinTermMeta(t, &norms[e * (kNormStride8 + 2)], true, *W1[(size_t)j], nd, S);
+      if (!firsts[set] && !plain(sums[set], t)) { loop(); return; }
+      P::addMeta(sums[set], firsts[set], t);
+    }
+  Ctxt meta = sums[0];
+  bool first = firsts[0];
+  if (bad && !firsts[1]) {
+    Ctxt t = sums[1];
+    if (Wf) {
+      if (!(t.primeSet == full)) { loop(); return; }
+      relinTermMeta(t, &norms[(size_t)(2 * d1) * (kNormStride8 + 2)], true, *Wf, nd, S);
+    }
+    if (!first && !plain(meta, t)) { loop(); return; }
+    P::addMeta(meta, first, t);
+  }
+  if (!(meta.primeSet == full)) { loop(); return; }   // only unrotated terms over S: the loop's result stays over S
   Ctxt out(pubKey, meta.ptxtSpace);
   out.primeSet = meta.primeSet; out.noiseBound = meta.noiseBound; out.intFactor = meta.intFactor;
   out.ratFactor = meta.ratFactor; out.ptxtMag = meta.ptxtMag;
