@@ -342,6 +342,121 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restric
   hb1_cp_wait<0>();
 }
 
+// Rescale of a multiplication's four operand parts and their tensor product in one forward blk pass (scaleDownToSet of
+// a0, a1, b0, b1, then Ctxt::tensorProduct, src/Ctxt.cpp:1563-1608).  nitems counts operand pairs; src[4*it + k] is the
+// coefficient-side tile of part k (a0, a1, b0, b1) left by the conversion, dst[4*it + k] that part's rows.  A unit
+// (row, group of 16 blocks, item) runs the forward blk phase of the four parts in turn with the twiddles loaded once,
+// applies the subscale epilogue of k1_fwd_blk (v = (old - x) * P^-1, lazy in [0,4q)) and stores, canonical,
+//   a0 <- a0*b0,   a1 <- a0*b1 + a1*b0,   b0 <- a1*b1
+// and b1 <- b1' (lazy, as the separate rescale leaves it).  The pass-2 positions of a thread do not depend on the part, so
+// the combination is thread-local: a0', a1' and then a1'*b0' mod q wait in per-thread slots V of shared memory (held in
+// registers they take the kernel past 255 registers and into local memory).  Part k's old values are read before the unit
+// stores anything over them: o0 goes out with part 2 into a0 (read by part 0), o1, o2 and b1' with part 3 into a1, b0 and
+// b1 (read by parts 1, 2, 3).  Part k stages in S[k & 1] and prefetches part k+1 (part 0 of the next unit after part 3)
+// while it computes.  The part loop stays rolled: four unrolled copies of the network (180 KB of code) ran from the
+// instruction cache's misses at a third of the speed.
+// smem: S[2][HB1_STAGE] | O[16][256] | TW1[256] | V[3][16][256]
+template <bool SP>
+__global__ void __launch_bounds__(256, 1) k1_fwd_blk_tensor(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT Hb1BlkJob J) {
+  HB_SMEM_DECL
+  u64* S = HB_SMEM;
+  u64* O = S + 2 * HB1_STAGE;
+  ulonglong2* TW1 = (ulonglong2*)(O + 16 * 256);
+  u64* V = (u64*)(TW1 + 256);
+  const int tid = threadIdx.x;
+  const int n1 = J.logN - 8;
+  const int G = 1 << (n1 - 4);
+  const long U = (long)J.rows.n * G * J.nitems;
+  const long ubeg = U * blockIdx.x / gridDim.x, uend = U * (blockIdx.x + 1) / gridDim.x;
+  if (ubeg >= uend) return;
+  const int blk1 = tid >> 4, lo = tid & 15;
+  const int hi = tid >> 4, blk2 = tid & 15;
+  const unsigned hrev = hb1_brev4(hi);
+  const int own = blk1 * HB1_BS + lo;   // + HB1_RS * r
+  u64* const Vt = V + tid;              // slot j of position l: Vt[j * 4096 + l * 256]
+  Hb1TwPtr tw1;
+  tw1.p[0] = TW1 + blk1 * 16; tw1.p[1] = tw1.p[0] + 1; tw1.p[2] = tw1.p[0] + 3; tw1.p[3] = tw1.p[0] + 7;
+
+  auto prefetch = [&](u64* Sn, const Hb1Unit& x, int k) {
+    const unsigned b = hb_brev((x.ug << 4) + blk1, n1);
+    const u64* src = J.src[4 * x.it + k] + ((size_t)J.rows.prime[x.rowi] << J.logN) + ((size_t)b << 8) + lo;
+    hb1_unroll<16>([&](auto r) { hb1_cp8(Sn + own + HB1_RS * r, src + 16 * r); });
+  };
+  Hb1Unit cur = hb1_unit(ubeg, G, J.nitems);
+  prefetch(S, cur, 0);
+  hb1_cp_commit();
+  int key = -1;
+  u64 q = 0, sc = 0, sc_s = 0, c64 = 0, c64_s = 0, one_s = 0;
+  Hb1Mod M; M.nq = 0; M.qb = 0; M.qb2 = 0; M.qt = 0; M.qsh = 0;
+  Hb1TwReg tw2;
+  for (long u = ubeg; u < uend; u++) {
+    if (cur.rowi * G + cur.ug != key) {   // new (row, block group): reload modulus and twiddles
+      key = cur.rowi * G + cur.ug;
+      const HbPrimeDev P = primes[J.rows.prime[cur.rowi]];
+      q = P.q; M.nq = P.nq; M.qb = P.qb; M.qb2 = P.qb + P.qb; M.qt = P.qt; M.qsh = P.qsh;
+      c64 = P.c64; c64_s = P.c64_s; one_s = P.one_s;
+      sc = J.scal[cur.rowi]; sc_s = J.scal_s[cur.rowi];
+      const unsigned b1 = hb_brev((cur.ug << 4) + blk1, n1), b2 = hb_brev((cur.ug << 4) + blk2, n1);
+      if (lo < 15) {  // entry e = (1<<k)-1+g of block blk1
+        int e = lo, k = e >= 7 ? 3 : (e >= 3 ? 2 : (e >= 1 ? 1 : 0));
+        int g = e - ((1 << k) - 1);
+        TW1[blk1 * 16 + e] = P.fw[((size_t)1 << (n1 + k)) + ((size_t)b1 << k) + g];
+      }
+      tw2.load([&](int k, int g) { return P.fw[((size_t)1 << (n1 + 4 + k)) + ((size_t)b2 << (4 + k)) + ((size_t)hi << k) + g]; });
+      __syncthreads();  // TW1 visible (the previous unit's trailing barrier ordered its last use)
+    }
+    const size_t doff = ((size_t)J.rows.prime[cur.rowi] << J.logN) + (cur.ug << 4) + blk2;
+    u64* const* dst = J.dst + 4 * cur.it;
+    const bool more = u + 1 < uend;
+    const Hb1Unit nxt = more ? hb1_unit_next(cur, G, J.nitems) : cur;
+#pragma unroll 1
+    for (int k = 0; k < 4; k++) {
+      u64* Sb = S + (k & 1) * HB1_STAGE;
+      const u64* old = dst[k] + doff;
+      hb1_unroll<16>([&](auto l) { hb1_cp8(O + l * 256 + tid, old + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1)); });
+      hb1_cp_commit();
+      if (k < 3) prefetch(S + ((k + 1) & 1) * HB1_STAGE, cur, k + 1);
+      else if (more) prefetch(S, nxt, 0);
+      hb1_cp_commit();
+      hb1_cp_wait<2>();   // this part's inputs have landed (issued one part ago)
+      u64 a[16];
+      hb1_unroll<16>([&](auto r) { a[r] = Sb[own + HB1_RS * r]; });
+      hb1_r16_fwd<SP>(a, tw1, M);
+      hb1_unroll<16>([&](auto r) { Sb[own + HB1_RS * r] = a[r]; });
+      __syncthreads();
+      hb1_unroll<16>([&](auto l) { a[l] = Sb[blk2 * HB1_BS + HB1_RS * hi + l]; });
+      hb1_r16_fwd<SP>(a, tw2, M);
+      hb1_cp_wait<1>();   // old values of this part have landed
+      hb1_unroll<16>([&](auto l) {   // (old - x) * P^-1 in [0,4q), x in [0, 8q + 2^32), old < 4q
+        a[l] = hb1_shoup4<SP>(O[l * 256 + tid] - a[l] + (M.qb2 + M.qb), sc, sc_s, M);
+      });
+      if (k < 2) {   // a0', a1'
+        hb1_unroll<16>([&](auto l) { Vt[k * 4096 + l * 256] = a[l]; });
+      } else if (k == 2) {   // b0': o0 = a0'*b0' out, a1'*b0' kept
+        hb1_unroll<16>([&](auto l) {
+          const size_t o = doff + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1);
+          const u64 x0 = Vt[l * 256], x1 = Vt[4096 + l * 256], v = a[l];
+          dst[0][o] = hb_reduce128(__umul64hi(x0, v), x0 * v, q, c64, c64_s, one_s);
+          Vt[2 * 4096 + l * 256] = hb_reduce128(__umul64hi(x1, v), x1 * v, q, c64, c64_s, one_s);
+        });
+      } else {   // b1': o1 = a0'*b1' + a1'*b0', o2 = a1'*b1'
+        hb1_unroll<16>([&](auto l) {
+          const size_t o = doff + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1);
+          const u64 x0 = Vt[l * 256], x1 = Vt[4096 + l * 256], v = a[l];
+          u64 h = 0, w = Vt[2 * 4096 + l * 256];
+          hb1_mac128(h, w, x0, v);
+          dst[1][o] = hb_reduce128(h, w, q, c64, c64_s, one_s);
+          dst[2][o] = hb_reduce128(__umul64hi(x1, v), x1 * v, q, c64, c64_s, one_s);
+          dst[3][o] = v;
+        });
+      }
+      __syncthreads();   // exchange reads of Sb / TW1 done before they are overwritten
+    }
+    cur = nxt;
+  }
+  hb1_cp_wait<0>();
+}
+
 // Inverse "blk" phase (bit-reversal + first 8 GS stages), same decomposition and pipelining.
 // smem: S[2][HB1_STAGE] | TW1[256]
 template <bool SP>

@@ -24,6 +24,10 @@
 
 typedef unsigned __int128 u128;
 
+static size_t blk_tensor_smem() {   // k1_fwd_blk_tensor: S[2][HB1_STAGE] | O[16][256] | TW1[256] | V[3][16][256]
+  return (2 * HB1_STAGE + 16 * 256 + 3 * 16 * 256) * sizeof(u64) + 256 * sizeof(ulonglong2);
+}
+
 // ------------------------------------------------------------------------------------------
 // errors
 static thread_local char g_err[512] = "";
@@ -331,6 +335,8 @@ static int ctx_build(hb_ctx* c, hb_ctx** out, int device, uint64_t m, int nprime
   HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
   HB_CUDA(cudaFuncSetAttribute(k1_inv_blk<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
   HB_CUDA(cudaFuncSetAttribute(k1_inv_blk<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
+  HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk_tensor<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blk_tensor_smem()));
+  HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk_tensor<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blk_tensor_smem()));
 #endif
   *out = c;
   return HB_OK;
@@ -847,6 +853,26 @@ static int launch_blk_v1(hb_ctx* c, int dir, const u64* const* src, u64* const* 
     const bool sp = all_special(c);
     if (dir > 0) { if (sp) HB_LAUNCH(k1_fwd_blk<true>, grid, dim3(256), smem, c->stream, c->d_primes, J); else HB_LAUNCH(k1_fwd_blk<false>, grid, dim3(256), smem, c->stream, c->d_primes, J); HB_TRY(post_launch(c, epi == 1 ? "k1_fwd_blk_subscale" : (epi == 3 ? "k1_fwd_blk_digits" : "k1_fwd_blk"), (u64)(epi == 1 ? 3 : 2) * nr * nitems * c->N * 8)); }
     else { if (sp) HB_LAUNCH(k1_inv_blk<true>, grid, dim3(256), smem, c->stream, c->d_primes, J); else HB_LAUNCH(k1_inv_blk<false>, grid, dim3(256), smem, c->stream, c->d_primes, J); HB_TRY(post_launch(c, "k1_inv_blk", (u64)2 * nr * nitems * c->N * 8)); }
+  }
+  return HB_OK;
+}
+// the rescale of nitems operand pairs (src / dst: 4 per pair, a0 a1 b0 b1) fused with their tensor product: k1_fwd_blk_tensor
+static int launch_blk_tensor_v1(hb_ctx* c, const u64* const* src, u64* const* dst, int nitems, const int32_t* idx, int n, const u64* scal) {
+  const int n1 = c->logN - 8;
+  for (int r0 = 0; r0 < n; r0 += HB_MAXROWS) {
+    int nr = std::min(HB_MAXROWS, n - r0);
+    Hb1BlkJob J; memset(&J, 0, sizeof(J));
+    J.logN = c->logN; J.epi = 1; J.lazy = 1;
+    fill_rows(J.rows, idx + r0, nr);
+    for (int i = 0; i < nr; i++) { J.scal[i] = scal[r0 + i]; J.scal_s[i] = h_shoup(scal[r0 + i], c->q[idx[r0 + i]]); }
+    J.nitems = nitems;
+    for (int i = 0; i < 4 * nitems; i++) { J.src[i] = src[i]; J.dst[i] = dst[i]; }
+    long units = (long)nr * nitems << (n1 - 4);
+    dim3 grid((unsigned)std::min<long>(units, std::max(1, c->resident_ctas / 2)));   // persistent CTAs, one per SM
+    pre_launch(c);
+    if (all_special(c)) HB_LAUNCH(k1_fwd_blk_tensor<true>, grid, dim3(256), blk_tensor_smem(), c->stream, c->d_primes, J);
+    else HB_LAUNCH(k1_fwd_blk_tensor<false>, grid, dim3(256), blk_tensor_smem(), c->stream, c->d_primes, J);
+    HB_TRY(post_launch(c, "k1_fwd_blk_tensor", (u64)12 * nr * nitems * c->N * 8));   // 4 tiles + 4 old rows read, 4 rows written
   }
   return HB_OK;
 }
@@ -1615,18 +1641,25 @@ extern "C" int hb_add_primes_norm(hb_poly* const* polys, int nitems, const int32
 }
 // norms (optional, [nitems]): canonical-embedding norm of delta/P (the "fdelta" of Ctxt::modDownToSet, src/Ctxt.cpp:476-505)
 // lazy: results only reduced to [0,4q) (register kernels only; for consumers inside the fused ciphertext paths)
-static int scale_down_impl(hb_poly* const* polys, int nitems, const int32_t* cur, int ncur, const int32_t* keep, int nkeep, uint64_t ptxt_space, double* norms, int lazy = 0) {
-  hb_ctx* c = nullptr; HB_TRY(check_polys(polys, nitems, &c, "hb_scale_down"));
+// the checks and prime sets of scaleDownToSet: diff = cur \ keep (dropped), kept = cur & keep, sc = prod(diff)^-1 on the kept rows;
+// nothing to do when diff comes back empty
+static int scale_down_sets(hb_ctx* c, const int32_t* cur, int ncur, const int32_t* keep, int nkeep, uint64_t ptxt_space,
+                           std::vector<int32_t>& diff, std::vector<int32_t>& kept, std::vector<u64>& sc) {
   HB_TRY(check_idx(c, cur, ncur, "hb_scale_down")); HB_TRY(check_idx(c, keep, nkeep, "hb_scale_down(keep)", true));
   if (ptxt_space < 1) return hb_fail(HB_ERR_BAD_ARG, "ptxtSpace must be at least 1");  // src/DoubleCRT.cpp:1472
-  std::vector<int32_t> diff, kept;
   for (int i = 0; i < ncur; i++) {
     bool k = std::find(keep, keep + nkeep, cur[i]) != keep + nkeep;
     (k ? kept : diff).push_back(cur[i]);
   }
   if (diff.empty()) return HB_OK;  // src/DoubleCRT.cpp:1468-1470
   if (kept.empty()) return hb_fail(HB_ERR_INDEX_SET, "scaleDownToSet: s and the index set must have some intersection");  // :1474-1476
-  std::vector<u64> sc; HB_TRY(scalars_by_primes(c, kept.data(), (int)kept.size(), diff.data(), (int)diff.size(), 1, sc));
+  return scalars_by_primes(c, kept.data(), (int)kept.size(), diff.data(), (int)diff.size(), 1, sc);
+}
+static int scale_down_impl(hb_poly* const* polys, int nitems, const int32_t* cur, int ncur, const int32_t* keep, int nkeep, uint64_t ptxt_space, double* norms, int lazy = 0) {
+  hb_ctx* c = nullptr; HB_TRY(check_polys(polys, nitems, &c, "hb_scale_down"));
+  std::vector<int32_t> diff, kept; std::vector<u64> sc;
+  HB_TRY(scale_down_sets(c, cur, ncur, keep, nkeep, ptxt_space, diff, kept, sc));
+  if (diff.empty()) return HB_OK;
   if (c->gen.on) {
     return for_items(nitems, [&](int i0, int nit) {
       u64* P[HB_MAXB]; u64* B[HB_MAXB]; ptrs_of(polys, i0, nit, P);
@@ -2925,6 +2958,29 @@ extern "C" int hb_relinearize(hb_poly* const* c0, hb_poly* const* c1, hb_poly* c
   return keyswitch_digits_impl(dig.data(), maxdig, nd, nitems, K.Sp.data(), (int)K.Sp.size(), evk_a, evk_b, c0, c1, K.scp.data(), 0, nullptr);
 }
 
+// bringToSet(S) of both operands and their tensor product on the register kernels: per chunk of pairs, the inverse blk phase
+// and the conversion of all four parts into adjacent scratch slots (4i .. 4i+3), then one k1_fwd_blk_tensor pass that finishes
+// the four rescales and writes the products over (a0, a1, b0) -- the rescaled a0, a1, b0 never make a round trip through HBM.
+// b1 receives its rescaled rows, as the separate rescale leaves them: the operands' rows after the call stay what they were.
+static int rescale_tensor_v1(hb_ctx* c, hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int nitems,
+                             const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space) {
+  std::vector<int32_t> diff, kept; std::vector<u64> sc;
+  HB_TRY(scale_down_sets(c, S_in, nS_in, S, nS, ptxt_space, diff, kept, sc));
+  if (diff.empty()) return hb_fail(HB_ERR_INDEX_SET, "hb_mul_relin_moddown: the fused rescale needs a dropped prime");
+  // ---- the rescale's arguments are checked (as scale_down_impl checks them) before its first launch
+  HB_TRY(ctx_scratch(c));
+  const int per = std::max(1, g_chunk / 4);   // pairs per chunk (the scratch holds HB_MAXB >= 4 parts)
+  for (int i0 = 0; i0 < nitems; i0 += per) {
+    const int nit = std::min(per, nitems - i0);
+    u64* P[HB_MAXB]; u64* tB[HB_MAXB];
+    for (int i = 0; i < nit; i++) { P[4 * i] = a0[i0 + i]->d; P[4 * i + 1] = a1[i0 + i]->d; P[4 * i + 2] = b0[i0 + i]->d; P[4 * i + 3] = b1[i0 + i]->d; }
+    tmp_ptrs(c, c->tmpB, 4 * nit, tB);
+    HB_TRY(conv_chunk(c, P, 4 * nit, diff.data(), (int)diff.size(), kept.data(), (int)kept.size(), ptxt_space));
+    HB_TRY(launch_blk_tensor_v1(c, (const u64* const*)tB, P, nit, kept.data(), (int)kept.size(), sc.data()));
+  }
+  return HB_OK;
+}
+
 extern "C" int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int nitems,
                                     const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space,
                                     hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk) {
@@ -2938,11 +2994,15 @@ extern "C" int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_p
   HB_TRY(check_idx(c, S, nS, "hb_mul_relin_moddown"));
   KsSets K; HB_TRY(ks_sets(c, S, nS, "breakIntoDigits", K));
   std::vector<hb_poly*> ka; HB_TRY(relin_key(c, K, evk_a, evk_b, ndig_evk, "hb_mul_relin_moddown", ka)); evk_a = ka.data();
-  std::vector<hb_poly*> allp;
-  for (int i = 0; i < nitems; i++) { allp.push_back(a0[i]); allp.push_back(a1[i]); allp.push_back(b0[i]); allp.push_back(b1[i]); }
-  HB_TRY(scale_down_impl(allp.data(), (int)allp.size(), S_in, nS_in, S, nS, ptxt_space, nullptr, c->gen.on ? 0 : 1));   // lazy rows: the tensor product reduces exactly
   // tensorProduct in place: (a0,a1,b0) <- (a0*b0, a0*b1+a1*b0, a1*b1)   (src/Ctxt.cpp:1563-1608)
-  HB_TRY(hb_tensor(a0, a1, b0, b1, a0, a1, b0, nitems, S, nS));
+  if (v1_blk_ok(c) && !c->gen.on && nS < nS_in) {   // S is a subset of S_in: something is dropped
+    HB_TRY(rescale_tensor_v1(c, a0, a1, b0, b1, nitems, S_in, nS_in, S, nS, ptxt_space));
+  } else {
+    std::vector<hb_poly*> allp;
+    for (int i = 0; i < nitems; i++) { allp.push_back(a0[i]); allp.push_back(a1[i]); allp.push_back(b0[i]); allp.push_back(b1[i]); }
+    HB_TRY(scale_down_impl(allp.data(), (int)allp.size(), S_in, nS_in, S, nS, ptxt_space, nullptr, c->gen.on ? 0 : 1));   // lazy rows: the tensor product reduces exactly
+    HB_TRY(hb_tensor(a0, a1, b0, b1, a0, a1, b0, nitems, S, nS));
+  }
   // reLinearize (src/Ctxt.cpp:720-786)
   HB_TRY(hb_relinearize(a0, a1, b0, nitems, S, nS, evk_a, evk_b, ndig_evk));
   // drop the special primes again: modDownToSet(ctxtPrimes) (src/Ctxt.cpp:589-593)
