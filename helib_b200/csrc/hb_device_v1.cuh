@@ -861,9 +861,10 @@ __global__ void __launch_bounds__(256) k1_ks_inner(const HbPrimeDev* __restrict_
 
 // ------------------------------------------------------------------------------------------
 // Ctxt::tensorProduct (src/Ctxt.cpp:1563-1608), streaming form for power-of-two m: two adjacent coefficients per thread,
-// 128-bit loads and stores (the generic k_pointwise moves 8 bytes per access).  Inputs may be lazy (any 64-bit values:
-// the 128-bit products are reduced exactly); outputs canonical.  In place is allowed (every thread reads its four inputs
-// before it writes).     grid = (N / 512, nrows, nitems)
+// 128-bit loads and stores (the generic k_pointwise moves 8 bytes per access).  Inputs may be lazy up to 2^63.5: a0*b1 +
+// a1*b0 is summed in 128 bits before its one reduction, and two products of 64-bit values could pass 2^128 (the callers
+// pass values below 8q + 2^32 < 2^63); outputs canonical.  In place is allowed (every thread reads its four inputs before
+// it writes).     grid = (N / 512, nrows, nitems)
 struct Hb1TensorJob {
   u64 N;
   HbRows rows;
