@@ -886,3 +886,59 @@ __global__ void __launch_bounds__(256) k1_tensor(const HbPrimeDev* __restrict__ 
   hb1_st2(J.o2[it] + o, hb_mulmod(a1.x, b1.x, P), hb_mulmod(a1.y, b1.y, P));
 }
 
+// ------------------------------------------------------------------------------------------
+// innerProduct (src/Ctxt.cpp:2878-2893) before its one reLinearize: the tensor products of the pairs of every item, summed,
+//   o0 (+)= sum_j a0_j*b0_j,   o1 (+)= sum_j (a0_j*b1_j + a1_j*b0_j),   o2 (+)= sum_j a1_j*b1_j   (mod q)
+// in k1_tensor's streaming form (two adjacent coefficients per thread, 128-bit loads and stores), with the six 128-bit sums in
+// registers and each output written once.  Inputs may be lazy below 8q + 2^32 (the lazy scale-down); every word is reduced to
+// [0, q) on load, so each product is at most (q-1)^2 < 2^120 (q < 2^60) and 255 products plus one 64-bit value fit 128 bits:
+// o1 takes two products per pair, so every HB_TSUM_GROUP = 127 pairs the sums are reduced and carried on canonical.  The old
+// outputs (accumulate) may be any 64-bit values; the outputs are canonical.  a and b may alias (sums of squares); the
+// outputs alias no input.  Pair j of item t of the launch reads slot t*npairs + j.     grid = (N / 512, nrows, nitems)
+#define HB_TSUM_GROUP 127       // pairs per 128-bit accumulation
+#define HB_TSUM_SLOTS 128       // pair slots (pairs x items) per launch
+struct Hb1TensorSumJob {
+  u64 N;
+  HbRows rows;
+  int npairs, nitems, accumulate;
+  const u64* a0[HB_TSUM_SLOTS]; const u64* a1[HB_TSUM_SLOTS]; const u64* b0[HB_TSUM_SLOTS]; const u64* b1[HB_TSUM_SLOTS];
+  u64* o0[HB_MAXB]; u64* o1[HB_MAXB]; u64* o2[HB_MAXB];
+};
+__device__ __forceinline__ u64 hb1_canon(u64 x, const HbPrimeDev& P) {   // any x < 2^64 -> [0, q)
+  u64 r = x - __umul64hi(x, P.one_s) * P.q;   // [0, 2q)
+  return r >= P.q ? r - P.q : r;
+}
+__global__ void __launch_bounds__(256) k1_tensor_sum(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT Hb1TensorSumJob J) {
+  const int pi = J.rows.prime[blockIdx.y];
+  const HbPrimeDev P = primes[pi];
+  const int it = blockIdx.z;
+  const size_t o = (size_t)pi * (size_t)J.N + 2 * ((size_t)blockIdx.x * 256 + threadIdx.x);
+  u64 h0x = 0, l0x = 0, h0y = 0, l0y = 0, h1x = 0, l1x = 0, h1y = 0, l1y = 0, h2x = 0, l2x = 0, h2y = 0, l2y = 0;
+  if (J.accumulate) {
+    const ulonglong2 p0 = hb1_ld2(J.o0[it] + o), p1 = hb1_ld2(J.o1[it] + o), p2 = hb1_ld2(J.o2[it] + o);
+    l0x = p0.x; l0y = p0.y; l1x = p1.x; l1y = p1.y; l2x = p2.x; l2y = p2.y;
+  }
+  const int s0 = it * J.npairs;
+  for (int j0 = 0; j0 < J.npairs; j0 += HB_TSUM_GROUP) {
+    if (j0 > 0) {   // carry the group's sums on canonical
+      l0x = hb_reduce128(h0x, l0x, P); l0y = hb_reduce128(h0y, l0y, P); l1x = hb_reduce128(h1x, l1x, P);
+      l1y = hb_reduce128(h1y, l1y, P); l2x = hb_reduce128(h2x, l2x, P); l2y = hb_reduce128(h2y, l2y, P);
+      h0x = h0y = h1x = h1y = h2x = h2y = 0;
+    }
+    const int j1 = J.npairs - j0 < HB_TSUM_GROUP ? J.npairs : j0 + HB_TSUM_GROUP;
+    for (int j = j0; j < j1; j++) {
+      const int s = s0 + j;
+      const ulonglong2 A0 = hb1_ld2(J.a0[s] + o), A1 = hb1_ld2(J.a1[s] + o), B0 = hb1_ld2(J.b0[s] + o), B1 = hb1_ld2(J.b1[s] + o);
+      const u64 a0x = hb1_canon(A0.x, P), a0y = hb1_canon(A0.y, P), a1x = hb1_canon(A1.x, P), a1y = hb1_canon(A1.y, P);
+      const u64 b0x = hb1_canon(B0.x, P), b0y = hb1_canon(B0.y, P), b1x = hb1_canon(B1.x, P), b1y = hb1_canon(B1.y, P);
+      hb1_mac128(h0x, l0x, a0x, b0x); hb1_mac128(h0y, l0y, a0y, b0y);
+      hb1_mac128(h1x, l1x, a0x, b1x); hb1_mac128(h1x, l1x, a1x, b0x);
+      hb1_mac128(h1y, l1y, a0y, b1y); hb1_mac128(h1y, l1y, a1y, b0y);
+      hb1_mac128(h2x, l2x, a1x, b1x); hb1_mac128(h2y, l2y, a1y, b1y);
+    }
+  }
+  hb1_st2(J.o0[it] + o, hb_reduce128(h0x, l0x, P), hb_reduce128(h0y, l0y, P));
+  hb1_st2(J.o1[it] + o, hb_reduce128(h1x, l1x, P), hb_reduce128(h1y, l1y, P));
+  hb1_st2(J.o2[it] + o, hb_reduce128(h2x, l2x, P), hb_reduce128(h2y, l2y, P));
+}
+

@@ -126,6 +126,7 @@ struct hb_ctx {
   std::vector<hb_poly*> ks_a;   // a_i regenerated from a seeded evk_a for the key switch in flight (allocated on first use)
   std::vector<hb_poly*> bsgs;   // hb_bsgs_linear_map: rotated sums and their digits, HB_BSGS_GROUP*(2+ndig) polys (first use)
   std::vector<hb_poly*> block;  // hb_block_linear_map: rotations, rotated sums, digits and set-1 sums (first use)
+  std::vector<hb_poly*> ip;     // hb_inner_product: the s^2 part of each item of a chunk (first use)
 };
 // The row schedule of a seeded set (hb_poly_create_seeded): the ChaCha20 key, the rows, and in one device allocation the
 // first buffer of every schedule row (start[T+1]) and the exclusive row offset of every counted buffer (off[T*wmax]).
@@ -357,6 +358,7 @@ extern "C" void hb_ctx_destroy(hb_ctx* c) {
   for (hb_poly* p : c->ks_a) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->bsgs) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->block) { cudaFree(p->d); delete p; }
+  for (hb_poly* p : c->ip) { cudaFree(p->d); delete p; }
   for (HbTmap* sl : c->tmap_slabs) cudaFree(sl);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
   delete c;
@@ -2848,6 +2850,92 @@ extern "C" int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const*
   });
 }
 
+// The summed tensor products of hb_tensor_sum on checked arguments.  Pair j of item t is [t*npairs + j].  Power-of-two m with
+// N a multiple of 512 runs k1_tensor_sum, as many items per launch as fit HB_TSUM_SLOTS pair slots and, for more pairs than
+// that, later pair groups accumulating into the outputs.  Otherwise (general m, small N, HB_FORCE_V0) every pair is an
+// HB_PW_TENSOR pass into scratch (the first one straight into the outputs unless accumulating) and three ADDs, as hb_tensor's
+// generic path; that path needs canonical inputs.
+static int tensor_sum_impl(hb_ctx* c, hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int npairs,
+                           int nitems, const int32_t* idx, int n, hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int accumulate) {
+  if (!c->gen.on && c->N % 512 == 0 && !c->force_v0) {
+    const int ni = std::max(1, std::min(g_chunk, HB_TSUM_SLOTS / npairs));   // items per launch
+    const int pp = std::min(npairs, HB_TSUM_SLOTS / ni);                       // pairs per launch
+    for (int i0 = 0; i0 < nitems; i0 += ni) {
+      const int nit = std::min(ni, nitems - i0);
+      for (int j0 = 0; j0 < npairs; j0 += pp) {
+        const int np = std::min(pp, npairs - j0);
+        for (int r0 = 0; r0 < n; r0 += HB_MAXROWS) {
+          const int nr = std::min(HB_MAXROWS, n - r0);
+          Hb1TensorSumJob J; memset(&J, 0, sizeof(J));
+          J.N = c->N; J.npairs = np; J.nitems = nit; J.accumulate = accumulate || j0 > 0;
+          fill_rows(J.rows, idx + r0, nr);
+          for (int t = 0; t < nit; t++) {
+            for (int j = 0; j < np; j++) {
+              const size_t e = (size_t)(i0 + t) * npairs + j0 + j;
+              const int s = t * np + j;
+              J.a0[s] = a0[e]->d; J.a1[s] = a1[e]->d; J.b0[s] = b0[e]->d; J.b1[s] = b1[e]->d;
+            }
+            J.o0[t] = o0[i0 + t]->d; J.o1[t] = o1[i0 + t]->d; J.o2[t] = o2[i0 + t]->d;
+          }
+          pre_launch(c);
+          HB_LAUNCH(k1_tensor_sum, dim3((unsigned)(c->N / 512), nr, nit), dim3(256), 0, c->stream, c->d_primes, J);
+          HB_TRY(post_launch(c, "k1_tensor_sum", (u64)(4 * np + (J.accumulate ? 6 : 3)) * nr * nit * c->N * 8));
+        }
+      }
+    }
+    return HB_OK;
+  }
+  HB_TRY(ctx_scratch(c));
+  const int per = std::max(1, std::min(g_chunk, HB_MAXB / 3));   // items per chunk: three scratch slots each
+  for (int i0 = 0; i0 < nitems; i0 += per) {
+    const int nit = std::min(per, nitems - i0);
+    u64* O[3][HB_MAXB]; u64* T[HB_MAXB];
+    ptrs_of(o0, i0, nit, O[0]); ptrs_of(o1, i0, nit, O[1]); ptrs_of(o2, i0, nit, O[2]);
+    tmp_ptrs(c, c->tmpA, 3 * nit, T);
+    for (int j = 0; j < npairs; j++) {
+      u64 *A0[HB_MAXB], *A1[HB_MAXB], *B0[HB_MAXB], *B1[HB_MAXB];
+      for (int t = 0; t < nit; t++) {
+        const size_t e = (size_t)(i0 + t) * npairs + j;
+        A0[t] = a0[e]->d; A1[t] = a1[e]->d; B0[t] = b0[e]->d; B1[t] = b1[e]->d;
+      }
+      const bool direct = j == 0 && !accumulate;
+      PwArgs A; memset(&A, 0, sizeof(A));
+      A.op = HB_PW_TENSOR; A.dst = direct ? O[0] : T; A.dst1 = direct ? O[1] : T + nit; A.dst2 = direct ? O[2] : T + 2 * nit;
+      A.a = (const u64* const*)A0; A.b = (const u64* const*)A1; A.cc = (const u64* const*)B0; A.d = (const u64* const*)B1;
+      HB_TRY(launch_pw(c, A, nit, idx, n));
+      if (direct) continue;
+      for (int k = 0; k < 3; k++) {
+        PwArgs B; memset(&B, 0, sizeof(B));
+        B.op = HB_PW_ADD; B.dst = O[k]; B.a = (const u64* const*)(T + k * nit);
+        HB_TRY(launch_pw(c, B, nit, idx, n));
+      }
+    }
+  }
+  return HB_OK;
+}
+// outputs written while the inputs `in` are read: distinct, and aliasing none of them
+static int check_outputs(const std::set<const hb_poly*>& in, std::initializer_list<hb_poly* const*> outs, int nitems, const char* who) {
+  std::set<const hb_poly*> out;
+  for (hb_poly* const* o : outs) out.insert(o, o + nitems);
+  if (out.size() != outs.size() * (size_t)nitems) return hb_fail(HB_ERR_BAD_ARG, "%s: the outputs must be distinct polynomials", who);
+  for (const hb_poly* p : out) if (in.count(p)) return hb_fail(HB_ERR_BAD_ARG, "%s: an output aliases an input", who);
+  return HB_OK;
+}
+extern "C" int hb_tensor_sum(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int npairs, int nitems,
+                             const int32_t* idx, int n, hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int accumulate) {
+  static const char* who = "hb_tensor_sum";
+  if (npairs <= 0 || nitems <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: npairs and nitems must be positive", who);
+  if (accumulate != 0 && accumulate != 1) return hb_fail(HB_ERR_BAD_ARG, "%s: accumulate must be 0 or 1", who);
+  hb_ctx* c = nullptr;
+  const int np = npairs * nitems;
+  HB_TRY(check_polys(a0, np, &c, who)); HB_TRY(check_polys(a1, np, &c, who)); HB_TRY(check_polys(b0, np, &c, who)); HB_TRY(check_polys(b1, np, &c, who));
+  HB_TRY(check_polys(o0, nitems, &c, who)); HB_TRY(check_polys(o1, nitems, &c, who)); HB_TRY(check_polys(o2, nitems, &c, who));
+  HB_TRY(check_idx(c, idx, n, who));
+  std::set<const hb_poly*> in(a0, a0 + np); in.insert(a1, a1 + np); in.insert(b0, b0 + np); in.insert(b1, b1 + np);
+  HB_TRY(check_outputs(in, {o0, o1, o2}, nitems, who));
+  return tensor_sum_impl(c, a0, a1, b0, b1, npairs, nitems, idx, n, o0, o1, o2, accumulate);
+}
+
 extern "C" int hb_automorph(hb_poly* const* dst, hb_poly* const* src, int nitems, const int32_t* idx, int n, uint64_t k) {
   hb_ctx* c = nullptr; HB_TRY(check_polys(dst, nitems, &c, "hb_automorph")); HB_TRY(check_polys(src, nitems, &c, "hb_automorph"));
   HB_TRY(check_idx(c, idx, n, "hb_automorph"));
@@ -3009,4 +3097,57 @@ extern "C" int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_p
   std::vector<hb_poly*> two;
   for (int i = 0; i < nitems; i++) { two.push_back(a0[i]); two.push_back(a1[i]); }
   return hb_scale_down(two.data(), (int)two.size(), K.Sp.data(), (int)K.Sp.size(), S, nS, ptxt_space);
+}
+
+// innerProduct (src/Ctxt.cpp:2878-2893) of operands already brought to one prime set: sum_j multLowLvl(a_j, b_j), then one
+// reLinearize and, if asked, the mod-down of hb_mul_relin_moddown.  Per chunk of items, k1_tensor_sum writes the summed
+// s^0 and s^1 parts straight into out0/out1 and the s^2 part into one scratch poly per item, which the relinearisation
+// consumes.  Operands over S_in with S a strict subset are brought to S first by the lazy scale-down, in place (each distinct
+// operand poly once, so a == b is allowed).
+extern "C" int hb_inner_product(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int npairs, int nitems,
+                                const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space,
+                                hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk, hb_poly* const* out0, hb_poly* const* out1, int moddown) {
+  static const char* who = "hb_inner_product";
+  if (npairs <= 0 || nitems <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: npairs and nitems must be positive", who);
+  if (moddown != 0 && moddown != 1) return hb_fail(HB_ERR_BAD_ARG, "%s: moddown must be 0 or 1", who);
+  hb_ctx* c = nullptr;
+  const int np = npairs * nitems;
+  HB_TRY(check_polys(a0, np, &c, who)); HB_TRY(check_polys(a1, np, &c, who)); HB_TRY(check_polys(b0, np, &c, who)); HB_TRY(check_polys(b1, np, &c, who));
+  HB_TRY(check_polys(out0, nitems, &c, who)); HB_TRY(check_polys(out1, nitems, &c, who));
+  HB_TRY(check_idx(c, S_in, nS_in, who)); HB_TRY(check_idx(c, S, nS, who));
+  for (int i = 0; i < nS; i++)
+    if (std::find(S_in, S_in + nS_in, S[i]) == S_in + nS_in)
+      return hb_fail(HB_ERR_INDEX_SET, "%s: the common set must be a subset of the operands' set (prime %d)", who, S[i]);
+  if (ptxt_space < 1) return hb_fail(HB_ERR_BAD_ARG, "%s: ptxt_space must be at least 1", who);
+  if (c->special.empty()) return hb_fail(HB_ERR_BAD_ARG, "%s: context has no special primes", who);
+  KsSets K; HB_TRY(ks_sets(c, S, nS, who, K));
+  const KsKeys key = {1, nullptr, evk_a, evk_b, "evk"};
+  HB_TRY(ks_check_keys(c, &key, 1, K.nd, ndig_evk, K.Sp, who));
+  std::set<const hb_poly*> in(a0, a0 + np); in.insert(a1, a1 + np); in.insert(b0, b0 + np); in.insert(b1, b1 + np);
+  HB_TRY(check_acc(in, &key, 1, K.nd, ndig_evk, out0, out1, nitems, who));
+  // ---- every argument is checked: nothing was launched before this point
+  std::vector<hb_poly*> ka; HB_TRY(ks_expand_a(c, evk_a, K.nd, K.Sp.data(), (int)K.Sp.size(), ka)); evk_a = ka.data();
+  if (nS < nS_in) {   // bringToSet(S) of every operand part (src/Ctxt.cpp:373-389), lazy rows: the tensor sum reduces on load
+    std::vector<hb_poly*> parts; std::set<const hb_poly*> seen;
+    for (hb_poly* const* x : {a0, a1, b0, b1})
+      for (int i = 0; i < np; i++) if (seen.insert(x[i]).second) parts.push_back(x[i]);
+    HB_TRY(scale_down_impl(parts.data(), (int)parts.size(), S_in, nS_in, S, nS, ptxt_space, nullptr, c->gen.on ? 0 : 1));
+  }
+  const int G = std::min(nitems, c->chunk);
+  while ((int)c->ip.size() < G) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->ip.push_back(p); }
+  std::vector<hb_poly*> two;
+  for (int i0 = 0; i0 < nitems; i0 += G) {
+    const int nit = std::min(G, nitems - i0);
+    const size_t e = (size_t)i0 * npairs;
+    g_chunk = c->chunk;
+    HB_TRY(tensor_sum_impl(c, a0 + e, a1 + e, b0 + e, b1 + e, npairs, nit, S, nS, out0 + i0, out1 + i0, c->ip.data(), 0));
+    // reLinearize (src/Ctxt.cpp:720-786) over S | special: the fused or the step-by-step path of hb_relinearize
+    HB_TRY(hb_relinearize(out0 + i0, out1 + i0, c->ip.data(), nit, S, nS, evk_a, evk_b, ndig_evk));
+    if (!moddown) continue;
+    // modDownToSet(S) of the result, as hb_mul_relin_moddown ends (src/Ctxt.cpp:589-593)
+    two.clear();
+    for (int i = 0; i < nit; i++) { two.push_back(out0[i0 + i]); two.push_back(out1[i0 + i]); }
+    HB_TRY(hb_scale_down(two.data(), (int)two.size(), K.Sp.data(), (int)K.Sp.size(), S, nS, ptxt_space));
+  }
+  return HB_OK;
 }

@@ -346,6 +346,28 @@ class Engine:
         self._ck(self.lib.hb_mul_relin_moddown(_arr(a0), _arr(a1), _arr(b0), _arr(b1), len(a0), pi, ni, ps, ns,
                                                C.c_uint64(int(ptxt_space)), _arr(evk_a), _arr(evk_b), len(evk_a)))
 
+    def tensor_sum(self, a0, a1, b0, b1, o0, o1, o2, idx, accumulate=False):
+        """Per item t: the tensor products of its pairs (a0[t][j], a1[t][j]) x (b0[t][j], b1[t][j]), summed into
+        (o0[t], o1[t], o2[t]) on rows idx (hb_tensor_sum).  a0..b1: one list of pairs per item, all of one length."""
+        npairs = len(a0[0])
+        fl = [[p for item in x for p in item] for x in (a0, a1, b0, b1)]
+        assert all(len(item) == npairs for x in (a0, a1, b0, b1) for item in x)
+        a, p, n = _idx(idx)
+        self._ck(self.lib.hb_tensor_sum(_arr(fl[0]), _arr(fl[1]), _arr(fl[2]), _arr(fl[3]), npairs, len(a0), p, n,
+                                        _arr(o0), _arr(o1), _arr(o2), int(bool(accumulate))))
+
+    def inner_product(self, a0, a1, b0, b1, S_in, S, ptxt_space, evk_a, evk_b, out0, out1, moddown=True):
+        """Per item t: sum_j (a0,a1)[t][j] * (b0,b1)[t][j] brought to S, relinearised once into (out0[t], out1[t]) over
+        S | special, and with moddown over S (hb_inner_product).  Operands over S_in are brought to S in place."""
+        npairs = len(a0[0])
+        fl = [[p for item in x for p in item] for x in (a0, a1, b0, b1)]
+        assert all(len(item) == npairs for x in (a0, a1, b0, b1) for item in x)
+        x, pi, ni = _idx(S_in)
+        y, ps, ns = _idx(S)
+        self._ck(self.lib.hb_inner_product(_arr(fl[0]), _arr(fl[1]), _arr(fl[2]), _arr(fl[3]), npairs, len(a0), pi, ni, ps, ns,
+                                           C.c_uint64(int(ptxt_space)), _arr(evk_a), _arr(evk_b), len(evk_a),
+                                           _arr(out0), _arr(out1), int(bool(moddown))))
+
     def randomize(self, polys, idx, seed):
         """NTL::SetSeed(seed), then p.randomize() over rows idx for each p in polys, expanded on the device
         (hb_poly_randomize).  seed: the ZZ's little-endian magnitude bytes, or a non-negative int."""

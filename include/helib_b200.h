@@ -105,7 +105,8 @@ int hb_poly_randomize(hb_poly* const* polys, int npolys, const int32_t* idx, int
  * out[0..npolys) receive one handle per poly.  Runs the k_prg_count chain once and synchronises once.  Argument errors as
  * hb_poly_randomize (unsorted/duplicate idx, npolys <= 0, null seed with a length -> HB_ERR_BAD_ARG).
  * A seeded handle has no rows.  It is accepted in two places only: as an entry of evk_a of the key-switching entry points
- * (hb_keyswitch_digits, hb_keyswitch_digits_fused, hb_automorph_keyswitch_digits, hb_relinearize, hb_mul_relin_moddown),
+ * (hb_keyswitch_digits, hb_keyswitch_digits_fused, hb_automorph_keyswitch_digits, hb_relinearize, hb_mul_relin_moddown,
+ * hb_inner_product),
  * which regenerate the rows they read once per call into context scratch, and as `seeded` of hb_poly_expand.  Everything
  * else returns HB_ERR_BAD_ARG for it before launching anything; a key switch that needs a row outside the seeded set
  * returns HB_ERR_INDEX_SET.  hb_poly_destroy each handle; the shared schedule is freed with the last one and its bytes
@@ -298,6 +299,14 @@ int hb_block_linear_map_norm(hb_poly* const* digits, int maxdig, int nitems, con
 /* Ctxt::tensorProduct of two canonical 2-part ciphertexts (src/Ctxt.cpp:1563-1608) */
 int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1,
               hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int nitems, const int32_t* idx, int n);
+/* The tensor products of npairs pairs per item, summed (Ctxt::multLowLvl's tensorProduct followed by innerProduct's +=,
+ * src/Ctxt.cpp:2878-2893, for operands already at one prime set).  Pair j of item t is [t*npairs + j]; on rows idx:
+ *   o0 (+)= sum_j a0_j*b0_j,  o1 (+)= sum_j (a0_j*b1_j + a1_j*b0_j),  o2 (+)= sum_j a1_j*b1_j   (mod q)
+ * accumulate = 0 overwrites the outputs.  Inputs are read-only and may alias each other (a == b: sums of squares); on the
+ * register path (power-of-two m, N a multiple of 512) they may be lazy below 8q + 2^32.  Outputs are canonical.
+ * npairs or nitems <= 0, accumulate not 0/1, or an output aliasing an input or another output -> HB_ERR_BAD_ARG. */
+int hb_tensor_sum(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int npairs, int nitems,
+                  const int32_t* idx, int n, hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int accumulate);
 /* DoubleCRT::automorph (src/DoubleCRT.cpp:1160-1202): dst[j] = src[idx(rep(j)*k mod m)], dst != src */
 int hb_automorph(hb_poly* const* dst, hb_poly* const* src, int nitems, const int32_t* idx, int n, uint64_t k);
 
@@ -350,6 +359,17 @@ int hb_relinearize(hb_poly* const* c0, hb_poly* const* c1, hb_poly* const* c2, i
 int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int nitems,
                          const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space,
                          hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk);
+/* hb_inner_product: innerProduct (src/Ctxt.cpp:2878-2893) of nitems vectors of npairs pairs, the batched form of
+ * hb_mul_relin_moddown for sums: pair j of item t is (a0,a1),(b0,b1)[t*npairs + j], over S_in.  When S is a strict subset of
+ * S_in every operand part is first brought to S (its rows overwritten, as hb_mul_relin_moddown's operands); then the summed
+ * tensor products are relinearised once over S | special into (out0, out1), and with moddown = 1 modded down to S.  No
+ * relin_CKKS_adjust (the Ctxt layer applies it).  npairs or nitems <= 0, moddown not 0/1, too few matrix columns, an output
+ * aliasing an input, a key or another output, or a seeded handle other than in evk_a -> HB_ERR_BAD_ARG; S not within S_in
+ * or not within the ctxt primes, or a seeded evk_a without a needed row -> HB_ERR_INDEX_SET; all checked before any launch.
+ * Stream-ordered, no synchronisation; after the first call, a call of the same shape allocates nothing. */
+int hb_inner_product(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int npairs, int nitems,
+                     const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space,
+                     hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk, hb_poly* const* out0, hb_poly* const* out1, int moddown);
 
 #ifdef __cplusplus
 }

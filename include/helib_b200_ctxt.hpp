@@ -417,6 +417,14 @@ class Ctxt {
     if (&pubKey != &other_orig.pubKey) throw LogicError("Public key mismatch");
     if (isCKKS() && (ptxtSpace != 1 || other_orig.ptxtSpace != 1)) throw LogicError("Plaintext spaces incompatible");
     Ctxt other = other_orig;
+    bringToCommonSet(other);
+    Ctxt tmp(pubKey, ptxtSpace);
+    tmp.tensorProduct(*this, other);
+    *this = tmp;
+  }
+  // multLowLvl's preparation of the two operands (src/Ctxt.cpp:1717-1747): equal plaintext spaces, then both brought to the
+  // common prime set that getSet4Size picks for the product
+  void bringToCommonSet(Ctxt& other) {
     if (!isCKKS()) {   // equalize plaintext spaces (src/Ctxt.cpp:1717-1725); reducePtxtSpace also reduces intFactor
       long g = std::gcd(ptxtSpace, other.ptxtSpace);
       if (g <= 1) throw LogicError("Plaintext spaces are co-prime");
@@ -432,9 +440,6 @@ class Ctxt {
     lastCommonPrimeSet = common; lastLo = lo; lastHi = hi;
     bringToSet(common);
     other.bringToSet(common);
-    Ctxt tmp(pubKey, ptxtSpace);
-    tmp.tensorProduct(*this, other);
-    *this = tmp;
   }
   // ---- linear operations (addConstant / multByConstant: BGV branches only)
   void negate() { for (auto& part : parts) part.dcrt.Negate(); }   // src/Ctxt.cpp:1190-1194
@@ -1162,6 +1167,81 @@ inline void MatMul1DBSGS(Ctxt& ctxt, long gen, long D, const std::vector<BsgsDia
   out.parts.emplace_back(a0, SKHandle());
   out.parts.emplace_back(a1, SKHandle(1, 1, keyID));
   ctxt = out;
+}
+
+// ---- innerProduct (src/Ctxt.cpp:2878-2893) ----------------------------------------------------------------------------
+// result = sum_i v1[i] * v2[i] over the first min(|v1|, |v2|) pairs, relinearised once at the end.  Every pair is prepared as
+// multLowLvl prepares it (copies brought to the common prime set getSet4Size picks).  When every prepared operand is a 2-part
+// canonical ciphertext under one key, every pair lands on one prime set with one ptxtSpace, and the terms sum as a plain add
+// (BGV: one intFactor; CKKS: one ratFactor), one hb_tensor_sum call forms the 3-part sum and the loop's metadata is replayed
+// term by term through tensorProduct and addCtxt's metadata steps.  Otherwise the transcribed loop (multLowLvl, +=) runs.
+// Either way the mirror's own reLinearize finishes, so the result has the loop's bits and metadata.
+inline void innerProduct(Ctxt& result, const std::vector<Ctxt>& v1, const std::vector<Ctxt>& v2) {
+  using P = BasicAutomorphPrecon;
+  const size_t n = std::min(v1.size(), v2.size());
+  if (n == 0) {   // Ctxt::clear (include/helib/Ctxt.h:1347-1355)
+    result.parts.clear(); result.primeSet = result.context.getCtxtPrimes(); result.noiseBound = XD(0.0);
+    result.intFactor = 1; result.ratFactor = XD(1.0); result.ptxtMag = XD(1.0);
+    return;
+  }
+  auto loop = [&]() {
+    result = v1[0];
+    result.multLowLvl(v2[0]);
+    for (size_t i = 1; i < n; i++) { Ctxt tmp = v1[i]; tmp.multLowLvl(v2[i]); result += tmp; }
+    result.reLinearize();
+  };
+  auto meta_of = [](const Ctxt& c) {
+    Ctxt t(c.pubKey, c.ptxtSpace);
+    t.primeSet = c.primeSet; t.noiseBound = c.noiseBound; t.intFactor = c.intFactor; t.ratFactor = c.ratFactor; t.ptxtMag = c.ptxtMag;
+    return t;
+  };
+  // ---- the prepared pairs, and can one call reproduce the loop?
+  const KeyInfo& pubKey = result.pubKey;
+  const bool ckks = v1[0].isCKKS();
+  const long keyID = v1[0].getKeyID();
+  std::vector<Ctxt> x, y;
+  x.reserve(n); y.reserve(n);
+  Ctxt meta(pubKey, v1[0].ptxtSpace);
+  bool ok = true, first = true;
+  for (size_t i = 0; ok && i < n; i++) {
+    const Ctxt& a = v1[i];
+    const Ctxt& b = v2[i];
+    // the cases where multLowLvl returns early or throws take the loop
+    if (&a.pubKey != &pubKey || &b.pubKey != &pubKey || a.isEmpty() || b.isEmpty() || a.isCKKS() != ckks || b.isCKKS() != ckks ||
+        (ckks ? (a.ptxtSpace != 1 || b.ptxtSpace != 1) : std::gcd(a.ptxtSpace, b.ptxtSpace) <= 1)) { ok = false; break; }
+    x.push_back(a); y.push_back(b);
+    x.back().bringToCommonSet(y.back());
+    for (const Ctxt* c : {&x.back(), &y.back()})
+      ok = ok && c->parts.size() == 2 && c->inCanonicalForm(keyID) && c->getKeyID() == keyID;
+    if (!ok) break;
+    Ctxt t(pubKey, x.back().ptxtSpace);   // tensorProduct's metadata (its part loop has nothing to do on metadata-only operands)
+    t.tensorProduct(meta_of(x.back()), meta_of(y.back()));
+    if (!first && (!(t.primeSet == meta.primeSet) || t.ptxtSpace != meta.ptxtSpace || (!ckks && t.intFactor != meta.intFactor) ||
+                   (ckks && (t.ratFactor < meta.ratFactor || meta.ratFactor < t.ratFactor)))) { ok = false; break; }
+    P::addMeta(meta, first, t);
+  }
+  if (!ok) { loop(); return; }
+  // ---- the call
+  const IndexSet S = meta.primeSet;
+  std::vector<hb_poly*> a0, a1, b0, b1;
+  for (size_t i = 0; i < n; i++) {
+    a0.push_back(x[i].parts[0].dcrt.handle()); a1.push_back(x[i].parts[1].dcrt.handle());
+    b0.push_back(y[i].parts[0].dcrt.handle()); b1.push_back(y[i].parts[1].dcrt.handle());
+  }
+  DoubleCRT o0(result.context, S), o1(result.context, S), o2(result.context, S);
+  {
+    hb_poly* p0[1] = {o0.handle()}; hb_poly* p1[1] = {o1.handle()}; hb_poly* p2[1] = {o2.handle()};
+    auto Sv = S.vec();
+    check(hb_tensor_sum(a0.data(), a1.data(), b0.data(), b1.data(), (int)n, 1, Sv.data(), (int)Sv.size(), p0, p1, p2, 0));
+  }
+  const SKHandle s1(1, 1, keyID);
+  SKHandle s2; s2.mul(s1, s1);
+  Ctxt out = meta;
+  out.parts.emplace_back(o0, SKHandle());
+  out.parts.emplace_back(o1, s1);
+  out.parts.emplace_back(o2, s2);
+  result = out;
+  result.reLinearize();
 }
 
 // ---- BlockMatMul1DExec::mul's non-iterative branches (src/matmul.cpp:1663-1976) ------------------------------------
