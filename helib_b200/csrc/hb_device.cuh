@@ -1018,6 +1018,118 @@ __global__ void __launch_bounds__(HB_THREADS) k_ks_hoist(const HbPrimeDev* __res
   }
 }
 
+// Full linear map leaves (MatMulFullExec::rec_mul's last dimension, src/matmul.cpp:2141-2148, each leaf a hoisted
+// MatMul1DExec::mul, :1226-1283): k_ks_linmap's hoisted key switch with the roles changed.  All leaves share the amounts
+// and the matrices; leaf l of item it has its own digits, (c0, c1) over S and constants cst[l][t].  For every item:
+//   acc (+)= sum_l sum_t cst[l][t] * r_{l,t},  r_{l,t} = the hoisted rotation by k_t of leaf l (k_t == 1: scal*(c0, c1))
+//   BAD:  y_l (+)= sum_t cst1[l][t] * r_{l,t}   per leaf (HElib rotates and mods down every leaf's acc1 on its own)
+// The thread of position j holds LI leaves of one item: it loads each key word once for all of them.  Each inner product is
+// summed in 128 bits and reduced once; the products with the constants (below 2^120) go into one 128-bit sum per item
+// across leaves and amounts, reduced and carried before it holds 255 terms (its old value counts as one).  A y_l sum has
+// at most HB_LEAF_MAXAMT + 1 terms.  NULL constants are zero diagonals, skipped as MulAdd skips them.
+// Slot s = l*nitems + it holds leaf l of item it.  grid = (coefficient blocks, rows, items).  LI is 1, 2 or 4: at two CTAs
+// per SM (at most 128 registers) every instance keeps its state in registers, with no stack frame and no spill.
+#define HB_LEAF_PAIRS 32        // (item, leaf) pairs per launch: the leaf scratch of hb_full_linear_map_leaves
+#define HB_LEAF_MAXAMT 32       // amounts per launch
+struct HbLeafJob {
+  u64 N, m;
+  const int* rep; const int* irep;   // general m; null: power-of-two m
+  int ndig, nitems, nleaves, namt, accumulate, accumulate1;
+  HbRows rows;
+  u64 scal[HB_MAXROWS];              // P mod q on the rows of S, 0 on the special rows (addPrimesAndScale)
+  u64 k[HB_LEAF_MAXAMT];
+  const u64* evk_a[HB_LEAF_MAXAMT][HB_MAXDIG];
+  const u64* evk_b[HB_LEAF_MAXAMT][HB_MAXDIG];
+  const u64* cst[HB_LEAF_PAIRS * HB_LEAF_MAXAMT];    // [l*namt + t]; null: a zero diagonal
+  const u64* cst1[HB_LEAF_PAIRS * HB_LEAF_MAXAMT];   // the bad dimension's second set, same layout
+  const u64* dig[HB_LEAF_PAIRS][HB_MAXDIG];          // slot s
+  const u64* c0[HB_LEAF_PAIRS];
+  const u64* c1[HB_LEAF_PAIRS];
+  u64* y0[HB_LEAF_PAIRS];                            // BAD: the per-leaf sums, slot s
+  u64* y1[HB_LEAF_PAIRS];
+  u64* acc0[HB_LEAF_PAIRS];                          // [it]
+  u64* acc1[HB_LEAF_PAIRS];
+};
+template <int LI, bool BAD>
+__global__ void __launch_bounds__(HB_THREADS, 2) k_ks_leafmap(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT HbLeafJob J) {
+  const int pi = J.rows.prime[blockIdx.y];
+  const HbPrimeDev P = primes[pi];
+  const size_t N = (size_t)J.N;
+  const size_t off = (size_t)pi * N;
+  const u64 sc = J.scal[blockIdx.y];
+  const int it = blockIdx.z, ni = J.nitems, na = J.namt;
+  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < N; j += (size_t)gridDim.x * blockDim.x) {
+    const size_t o = off + j;
+    u64 h0 = 0, l0 = 0, h1 = 0, l1 = 0;
+    if (J.accumulate) { l0 = J.acc0[it][o]; l1 = J.acc1[it][o]; }
+    int terms = 1;   // terms in (h, l): the old value
+    const u64 rj = J.rep ? (u64)J.rep[j] : 2 * (u64)j + 1;   // m <= 2^20: rj*k < 2^41
+    for (int lg = 0; lg < J.nleaves; lg += LI) {
+      const int cnt = J.nleaves - lg < LI ? J.nleaves - lg : LI;
+      u64 yh0[LI], yl0[LI], yh1[LI], yl1[LI];
+#pragma unroll
+      for (int u = 0; u < LI; u++) {
+        yh0[u] = 0; yl0[u] = 0; yh1[u] = 0; yl1[u] = 0;
+        if (BAD && J.accumulate1 && u < cnt) { const int s = (lg + u) * ni + it; yl0[u] = J.y0[s][o]; yl1[u] = J.y1[s][o]; }
+      }
+      for (int t = 0; t < na; t++) {
+        bool any = false;
+#pragma unroll
+        for (int u = 0; u < LI; u++)
+          if (u < cnt) any = any || J.cst[(lg + u) * na + t] || (BAD && J.cst1[(lg + u) * na + t]);
+        if (!any) continue;
+        if (terms > 254 - LI) { l0 = hb_reduce128(h0, l0, P); l1 = hb_reduce128(h1, l1, P); h0 = 0; h1 = 0; terms = 1; }
+        terms += LI;
+        const u64 k = J.k[t];
+        u64 r0[LI], r1[LI];
+        if (k == 1) {   // no automorphism, no key switch: P*(c0, c1)
+#pragma unroll
+          for (int u = 0; u < LI; u++) {
+            r0[u] = 0; r1[u] = 0;
+            if (sc && u < cnt) {
+              const int s = (lg + u) * ni + it;
+              r0[u] = hb_mulmod(J.c0[s][o], sc, P); r1[u] = hb_mulmod(J.c1[s][o], sc, P);
+            }
+          }
+        } else {
+          const size_t g = off + (J.rep ? (size_t)J.irep[(rj * k) % J.m] : (size_t)(((rj * k) & (J.m - 1)) >> 1));
+          u64 p0h[LI], p0l[LI], p1h[LI], p1l[LI];
+#pragma unroll
+          for (int u = 0; u < LI; u++) {
+            p0h[u] = 0; p0l[u] = 0; p1h[u] = 0; p1l[u] = 0;
+            if (sc && u < cnt) hb_mac128(p0h[u], p0l[u], J.c0[(lg + u) * ni + it][g], sc);
+          }
+          for (int i = 0; i < J.ndig; i++) {
+            const u64 b = J.evk_b[t][i][o], a = J.evk_a[t][i][o];
+#pragma unroll
+            for (int u = 0; u < LI; u++)
+              if (u < cnt) { const u64 d = J.dig[(lg + u) * ni + it][i][g]; hb_mac128(p0h[u], p0l[u], d, b); hb_mac128(p1h[u], p1l[u], d, a); }
+          }
+#pragma unroll
+          for (int u = 0; u < LI; u++) { r0[u] = hb_reduce128(p0h[u], p0l[u], P); r1[u] = hb_reduce128(p1h[u], p1l[u], P); }
+        }
+#pragma unroll
+        for (int u = 0; u < LI; u++) {
+          if (u >= cnt) continue;
+          const u64* c = J.cst[(lg + u) * na + t];
+          if (c) { const u64 w = c[o]; hb_mac128(h0, l0, r0[u], w); hb_mac128(h1, l1, r1[u], w); }
+          if (BAD) {
+            const u64* c1 = J.cst1[(lg + u) * na + t];
+            if (c1) { const u64 w = c1[o]; hb_mac128(yh0[u], yl0[u], r0[u], w); hb_mac128(yh1[u], yl1[u], r1[u], w); }
+          }
+        }
+      }
+      if (BAD) {
+#pragma unroll
+        for (int u = 0; u < LI; u++)
+          if (u < cnt) { const int s = (lg + u) * ni + it; J.y0[s][o] = hb_reduce128(yh0[u], yl0[u], P); J.y1[s][o] = hb_reduce128(yh1[u], yl1[u], P); }
+      }
+    }
+    J.acc0[it][o] = hb_reduce128(h0, l0, P);
+    J.acc1[it][o] = hb_reduce128(h1, l1, P);
+  }
+}
+
 
 // ------------------------------------------------------------------------------------------
 // Canonical-embedding norm (noise metadata): max_j |f(zeta^(2j+1))|, zeta = e^(i*pi/N), in FP64.

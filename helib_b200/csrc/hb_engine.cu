@@ -127,6 +127,7 @@ struct hb_ctx {
   std::vector<hb_poly*> bsgs;   // hb_bsgs_linear_map: rotated sums and their digits, HB_BSGS_GROUP*(2+ndig) polys (first use)
   std::vector<hb_poly*> block;  // hb_block_linear_map: rotations, rotated sums, digits and set-1 sums (first use)
   std::vector<hb_poly*> ip;     // hb_inner_product: the s^2 part of each item of a chunk (first use)
+  std::vector<hb_poly*> leaf;   // hb_full_linear_map_leaves: cleaned leaves, their digits, per-leaf sums, final matrix (first use)
 };
 // The row schedule of a seeded set (hb_poly_create_seeded): the ChaCha20 key, the rows, and in one device allocation the
 // first buffer of every schedule row (start[T+1]) and the exclusive row offset of every counted buffer (off[T*wmax]).
@@ -358,6 +359,7 @@ extern "C" void hb_ctx_destroy(hb_ctx* c) {
   for (hb_poly* p : c->ks_a) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->bsgs) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->block) { cudaFree(p->d); delete p; }
+  for (hb_poly* p : c->leaf) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->ip) { cudaFree(p->d); delete p; }
   for (HbTmap* sl : c->tmap_slabs) cudaFree(sl);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
@@ -2817,6 +2819,213 @@ static int block_impl(hb_poly* const* digits, int maxdig, int nitems, const int3
                        acc0 + i0, acc1 + i0, acc_on, nf, (size_t)T));
   }
   return HB_OK;
+}
+
+// k_ks_leafmap with li leaves per thread (1, 2 or 4)
+template <int LI, bool BAD>
+static void leaf_launch1(hb_ctx* c, const dim3& g, const HbLeafJob& J) {
+  constexpr auto kern = k_ks_leafmap<LI, BAD>;   // one token for HB_LAUNCH
+  HB_LAUNCH(kern, g, dim3(HB_THREADS), 0, c->stream, c->d_primes, J);
+}
+template <bool BAD>
+static void leaf_launch(hb_ctx* c, int li, const dim3& g, const HbLeafJob& J) {
+  switch (li) {
+    case 1: leaf_launch1<1, BAD>(c, g, J); break;
+    case 2: leaf_launch1<2, BAD>(c, g, J); break;
+    default: leaf_launch1<4, BAD>(c, g, J); break;
+  }
+}
+// Full linear map leaves (SURVEY 8f-1): the last dimension of MatMulFullExec::rec_mul (src/matmul.cpp:2141-2148), every leaf
+// a hoisted MatMul1DExec::mul.  Per chunk of (item, leaf) pairs (slot l*nit + it): the cleanUp of the rotated leaves (a copy
+// into scratch and one batched mod-down), the digits of every leaf (one batched breakIntoDigits), then one k_ks_leafmap
+// pass per group of amounts and row chunk, all leaves of an item summed into its accumulators; in a bad dimension the
+// per-leaf sums are rotated by kfinal, modded down, decomposed and key-switched into the accumulators by bsgs_finish.
+static int full_leaves_impl(hb_poly* const* x0, hb_poly* const* x1, int nleaves, int nitems, const int32_t* ext,
+                            const int32_t* S, int nS, uint64_t ptxt_space, int namt, const uint64_t* k,
+                            hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* consts, hb_poly* const* consts1,
+                            uint64_t kfinal, hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                            hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms) {
+  static const char* who = "hb_full_linear_map_leaves";
+  hb_ctx* c = nullptr;
+  const bool bad = consts1 != nullptr;
+  if (nleaves <= 0 || nitems <= 0 || namt <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: nleaves, nitems and namt must be positive", who);
+  if (!k || !consts) return hb_fail(HB_ERR_BAD_ARG, "%s: no amounts", who);
+  HB_TRY(check_polys(x0, nitems * nleaves, &c, "hb_full_linear_map_leaves(x0)"));
+  HB_TRY(check_polys(x1, nitems * nleaves, &c, "hb_full_linear_map_leaves(x1)"));
+  for (int l = 0; ext && l < nleaves; l++) if (ext[l] != 0 && ext[l] != 1) return hb_fail(HB_ERR_BAD_ARG, "%s: ext[%d] must be 0 or 1", who, l);
+  HB_TRY(check_idx(c, S, nS, who));
+  if (ptxt_space < 1) return hb_fail(HB_ERR_BAD_ARG, "%s: ptxt_space must be at least 1", who);
+  if (c->special.empty()) return hb_fail(HB_ERR_BAD_ARG, "%s: context has no special primes", who);
+  KsSets K; HB_TRY(ks_sets(c, S, nS, who, K));
+  const int nd = K.nd;
+  if (nd > HB_MAXDIG) return hb_fail(HB_ERR_BAD_ARG, "%s: S has %d digits, at most %d are supported", who, nd, HB_MAXDIG);
+  HB_TRY(check_amounts(c, k, namt));
+  if (bad) HB_TRY(check_amounts(c, &kfinal, 1));
+  for (int i = 0; i < nleaves * namt; i++) if (consts[i]) HB_TRY(check_polys(consts + i, 1, &c, "hb_full_linear_map_leaves(consts)"));
+  for (int i = 0; bad && i < nleaves * namt; i++) if (consts1[i]) HB_TRY(check_polys(consts1 + i, 1, &c, "hb_full_linear_map_leaves(consts1)"));
+  HB_TRY(check_polys(acc0, nitems, &c, "hb_full_linear_map_leaves(acc0)")); HB_TRY(check_polys(acc1, nitems, &c, "hb_full_linear_map_leaves(acc1)"));
+  const KsKeys sets[2] = {{namt, k, evk_a, evk_b, "evk"}, {bad ? 1 : 0, &kfinal, evkf_a, evkf_b, "evkf"}};
+  bool seeded, seeded_f;
+  HB_TRY(ks_check_keys(c, sets, 1, nd, ndig_evk, K.Sp, who, &seeded));
+  HB_TRY(ks_check_keys(c, sets + 1, 1, nd, ndig_evk, K.Sp, who, &seeded_f));
+  std::set<const hb_poly*> in(x0, x0 + (size_t)nitems * nleaves);
+  in.insert(x1, x1 + (size_t)nitems * nleaves);
+  for (int i = 0; i < nleaves * namt; i++) { if (consts[i]) in.insert(consts[i]); if (bad && consts1[i]) in.insert(consts1[i]); }
+  HB_TRY(check_acc(in, sets, 2, nd, ndig_evk, acc0, acc1, nitems, who));
+  // ---- every argument is checked: nothing was launched before this point
+  const std::vector<int32_t>& Sp = K.Sp;
+  const int nSp = (int)Sp.size();
+  const std::vector<u64>& scp = K.scp;
+  const std::vector<u64> scx(Sp.size(), 1);   // the per-leaf sums are over S | special: extended form
+  const int T = bad ? 2 * nleaves : nleaves;   // norm entries per item
+  // chunks: at least 4 leaves (a thread's k_ks_leafmap<4> group) where the call has them, at most HB_LEAF_PAIRS pairs
+  const int lc = std::min(nleaves, std::max(4, HB_LEAF_PAIRS / std::min(nitems, HB_LEAF_PAIRS)));
+  const int ic = std::max(1, std::min(nitems, HB_LEAF_PAIRS / lc));
+  const int G = ic * lc;
+  const size_t need = (size_t)G * (2 + nd) + (bad ? 2 * (size_t)G : 0) + (bad && seeded_f ? nd : 0);
+  while (c->leaf.size() < need) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->leaf.push_back(p); }
+  hb_poly* const* XC0 = c->leaf.data();               // cleaned leaves; in a bad dimension then sigma_kfinal of the sums
+  hb_poly* const* XC1 = XC0 + G;
+  hb_poly* const* DG = XC1 + G;                        // digits, slot s at DG[s*nd ..]
+  hb_poly* const* Y0 = DG + (size_t)G * nd;            // the per-leaf sums of the bad dimension
+  hb_poly* const* Y1 = Y0 + G;
+  hb_poly* const* KF = Y1 + G;                         // kfinal's a_i, regenerated once per call when seeded
+  std::vector<hb_poly*> fa, fb;                        // kfinal's matrix once per leaf of a chunk (bsgs_finish's layout)
+  if (bad && kfinal != 1) {
+    std::vector<hb_poly*> ea(evkf_a, evkf_a + nd);
+    if (seeded_f) {
+      std::vector<hb_poly*> src; std::vector<u64*> dst;
+      for (int i = 0; i < nd; i++) if (evkf_a[i]->sched) { ea[(size_t)i] = KF[i]; src.push_back(evkf_a[i]); dst.push_back(KF[i]->d); }
+      HB_TRY(prg_expand(c, src.data(), dst.data(), (int)src.size(), Sp.data(), nSp, "key switch (evkf_a)"));
+    }
+    for (int l = 0; l < lc; l++) { fa.insert(fa.end(), ea.begin(), ea.end()); fb.insert(fb.end(), evkf_b, evkf_b + nd); }
+  }
+  const std::vector<uint64_t> kfv((size_t)lc, kfinal);
+  const int tmax = bsgs_tmax(nd, false);
+  const int achunk = seeded ? std::max(1, std::min(HB_LEAF_MAXAMT, HB_LINMAP_SEEDED / nd)) : HB_LEAF_MAXAMT;
+  std::vector<hb_poly*> L0((size_t)G), L1((size_t)G), cp0, cp1, sd, part1, dg((size_t)G * nd), list, ka, ysrc0, ysrc1, ydst0, ydst1;
+  std::vector<int> slot, sds;
+  for (int i0 = 0; i0 < nitems; i0 += ic) {
+    const int nit = std::min(ic, nitems - i0);
+    bool acc_on = accumulate != 0;
+    for (int l0 = 0; l0 < nleaves; l0 += lc) {
+      const int nl = std::min(lc, nleaves - l0), np = nl * nit;
+      // 1. cleanUp of the rotated leaves into scratch, and the digits of every leaf's part 1 over S
+      cp0.clear(); cp1.clear(); sd.clear(); sds.clear(); part1.clear();
+      for (int l = 0; l < nl; l++)
+        for (int it = 0; it < nit; it++) {
+          const int s = l * nit + it;
+          const size_t e = (size_t)(i0 + it) * nleaves + l0 + l;
+          if (ext && ext[l0 + l]) {
+            L0[(size_t)s] = XC0[s]; L1[(size_t)s] = XC1[s];
+            cp0.push_back(x0[e]); cp0.push_back(x1[e]); cp1.push_back(XC0[s]); cp1.push_back(XC1[s]); sds.push_back(s);
+          } else {
+            L0[(size_t)s] = x0[e]; L1[(size_t)s] = x1[e];
+          }
+          part1.push_back(L1[(size_t)s]);
+          for (int i = 0; i < nd; i++) dg[(size_t)s * nd + i] = DG[(size_t)s * nd + i];
+        }
+      std::vector<double> sdn(norms ? cp1.size() : 0), ldn(norms ? (size_t)np * nd : 0);
+      if (!cp1.empty()) {
+        HB_TRY(pw_simple(HB_PW_COPY, cp1.data(), cp0.data(), (int)cp1.size(), Sp.data(), nSp, nullptr, c));
+        HB_TRY(scale_down_impl(cp1.data(), (int)cp1.size(), Sp.data(), nSp, S, nS, ptxt_space, norms ? sdn.data() : nullptr));
+      }
+      int ndo = 0;
+      HB_TRY(break_into_digits_impl(part1.data(), np, S, nS, dg.data(), nd, &ndo, norms ? ldn.data() : nullptr));
+      if (norms) {
+        for (int s = 0; s < np; s++) {
+          double* o = norms + ((size_t)(i0 + s % nit) * T + l0 + s / nit) * (HB_MAXDIG + 2);
+          for (int i = 0; i < nd; i++) o[i] = ldn[(size_t)s * nd + i];
+        }
+        for (size_t r = 0; r < sds.size(); r++) {
+          const int s = sds[r];
+          double* o = norms + ((size_t)(i0 + s % nit) * T + l0 + s / nit) * (HB_MAXDIG + 2);
+          o[HB_MAXDIG] = sdn[2 * r]; o[HB_MAXDIG + 1] = sdn[2 * r + 1];
+        }
+      }
+      // 2. every leaf's rotations, weighted by its constants, into the accumulators (and the per-leaf sums)
+      for (int a0 = 0; a0 < namt; a0 += achunk) {
+        const int na = std::min(achunk, namt - a0);
+        list.clear(); slot.assign((size_t)na, -1);
+        for (int a = 0; a < na; a++)
+          if (k[a0 + a] != 1) { slot[(size_t)a] = (int)list.size(); list.insert(list.end(), evk_a + (size_t)(a0 + a) * ndig_evk, evk_a + (size_t)(a0 + a) * ndig_evk + nd); }
+        if (!list.empty()) HB_TRY(ks_expand_a(c, list.data(), (int)list.size(), Sp.data(), nSp, ka));
+        u64 item_rows = 0, shared_rows = 0;   // rows read (and written) per item and shared by the items, per row of the launch
+        for (int a = 0; a < na; a++) {
+          item_rows += (u64)nl * (k[a0 + a] == 1 ? 2 : nd + 1);
+          shared_rows += k[a0 + a] == 1 ? 0 : 2 * nd;
+          for (int l = 0; l < nl; l++) {
+            const size_t e = (size_t)(l0 + l) * namt + a0 + a;
+            shared_rows += (consts[e] != nullptr) + (bad && consts1[e] != nullptr);
+          }
+        }
+        item_rows += (acc_on ? 4 : 2) + (bad ? (u64)nl * (a0 > 0 ? 4 : 2) : 0);
+        for (int r0 = 0; r0 < nSp; r0 += HB_MAXROWS) {
+          const int nr = std::min(HB_MAXROWS, nSp - r0);
+          HbLeafJob J; memset(&J, 0, sizeof(J));
+          J.N = c->N; J.m = c->m;
+          if (c->gen.on) { J.rep = c->gen.d_rep; J.irep = c->gen.d_irep; }
+          J.ndig = nd; J.nitems = nit; J.nleaves = nl; J.namt = na; J.accumulate = acc_on ? 1 : 0; J.accumulate1 = a0 > 0 ? 1 : 0;
+          fill_rows(J.rows, Sp.data() + r0, nr);
+          for (int i = 0; i < nr; i++) J.scal[i] = scp[(size_t)(r0 + i)];
+          for (int a = 0; a < na; a++) {
+            const int t = a0 + a;
+            J.k[a] = k[t];
+            if (slot[(size_t)a] >= 0)
+              for (int i = 0; i < nd; i++) { J.evk_a[a][i] = ka[(size_t)slot[(size_t)a] + i]->d; J.evk_b[a][i] = evk_b[(size_t)t * ndig_evk + i]->d; }
+            for (int l = 0; l < nl; l++) {
+              const size_t e = (size_t)(l0 + l) * namt + t;
+              J.cst[l * na + a] = consts[e] ? consts[e]->d : nullptr;
+              if (bad) J.cst1[l * na + a] = consts1[e] ? consts1[e]->d : nullptr;
+            }
+          }
+          for (int s = 0; s < np; s++) {
+            J.c0[s] = L0[(size_t)s]->d; J.c1[s] = L1[(size_t)s]->d;
+            for (int i = 0; i < nd; i++) J.dig[s][i] = DG[(size_t)s * nd + i]->d;
+            if (bad) { J.y0[s] = Y0[s]->d; J.y1[s] = Y1[s]->d; }
+          }
+          for (int it = 0; it < nit; it++) { J.acc0[it] = acc0[i0 + it]->d; J.acc1[it] = acc1[i0 + it]->d; }
+          const int li = nl >= 4 ? 4 : nl >= 2 ? 2 : 1;
+          const dim3 g((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS), (unsigned)nr, (unsigned)nit);
+          pre_launch(c);
+          if (bad) leaf_launch<true>(c, li, g, J); else leaf_launch<false>(c, li, g, J);
+          HB_TRY(post_launch(c, "k_ks_leafmap", (item_rows * nit + shared_rows) * nr * c->N * 8));
+        }
+        acc_on = true;
+      }
+      if (!bad) continue;
+      // 3. every leaf's sum rotated by kfinal (smartAutomorph), added to its item's accumulators
+      double* nf = norms ? norms + ((size_t)i0 * T + nleaves + l0) * (HB_MAXDIG + 2) : nullptr;
+      if (kfinal == 1) {
+        HB_TRY(bsgs_finish(c, Y0, Y1, DG, nit, nl, kfv.data(), evkf_a, evkf_b, 0, nd, S, nS, Sp, 1, ptxt_space, scp, scx, tmax, false,
+                           acc0 + i0, acc1 + i0, acc_on, nf, (size_t)T));
+        continue;
+      }
+      ysrc0.assign(Y0, Y0 + np); ysrc1.assign(Y1, Y1 + np); ydst0.assign(XC0, XC0 + np); ydst1.assign(XC1, XC1 + np);
+      HB_TRY(hb_automorph(ydst0.data(), ysrc0.data(), np, Sp.data(), nSp, kfinal));
+      HB_TRY(hb_automorph(ydst1.data(), ysrc1.data(), np, Sp.data(), nSp, kfinal));
+      HB_TRY(bsgs_finish(c, XC0, XC1, DG, nit, nl, kfv.data(), fa.data(), fb.data(), nd, nd, S, nS, Sp, 1, ptxt_space, scp, scx, tmax, false,
+                         acc0 + i0, acc1 + i0, acc_on, nf, (size_t)T));
+    }
+  }
+  return HB_OK;
+}
+extern "C" int hb_full_linear_map_leaves(hb_poly* const* x0, hb_poly* const* x1, int nleaves, int nitems, const int32_t* ext,
+                                         const int32_t* S, int nS, uint64_t ptxt_space, int namt, const uint64_t* k,
+                                         hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* consts, hb_poly* const* consts1,
+                                         uint64_t kfinal, hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                                         hb_poly* const* acc0, hb_poly* const* acc1, int accumulate) {
+  return full_leaves_impl(x0, x1, nleaves, nitems, ext, S, nS, ptxt_space, namt, k, evk_a, evk_b, consts, consts1, kfinal, evkf_a, evkf_b,
+                          ndig_evk, acc0, acc1, accumulate, nullptr);
+}
+extern "C" int hb_full_linear_map_leaves_norm(hb_poly* const* x0, hb_poly* const* x1, int nleaves, int nitems, const int32_t* ext,
+                                              const int32_t* S, int nS, uint64_t ptxt_space, int namt, const uint64_t* k,
+                                              hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* consts, hb_poly* const* consts1,
+                                              uint64_t kfinal, hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                                              hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms) {
+  if (!norms) return hb_fail(HB_ERR_BAD_ARG, "hb_full_linear_map_leaves_norm: null output");
+  return full_leaves_impl(x0, x1, nleaves, nitems, ext, S, nS, ptxt_space, namt, k, evk_a, evk_b, consts, consts1, kfinal, evkf_a, evkf_b,
+                          ndig_evk, acc0, acc1, accumulate, norms);
 }
 
 extern "C" int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1,

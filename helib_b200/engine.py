@@ -641,10 +641,49 @@ def _engine_hoist(cls):
         self._ck(self.lib.hb_block_linear_map_norm(*args, out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
 
+    def full_linear_map_leaves(self, x0, x1, S, ks, evk_a, evk_b, consts, acc0, acc1, ext=None, consts1=None, kfinal=1,
+                               evkf_a=None, evkf_b=None, ptxt_space=1, accumulate=False, norms=False):
+        """acc (+)= the leaves of MatMulFullExec::rec_mul over S | special, for every item (hb_full_linear_map_leaves).
+        x0 / x1: per item, one Poly per leaf; ext: per leaf, whether it is over S | special (None: all over S); consts /
+        consts1: per leaf, one Poly (or None) per amount; consts1 (with kfinal and its matrix evkf_a / evkf_b) selects a
+        bad leaf dimension; evk_a / evk_b: per amount, the list of matrix Polys (None where the amount is 1).  norms=True
+        calls hb_full_linear_map_leaves_norm and returns its norms as [item][entry][10] (entry l: leaf l's cleanUp and
+        digits; nleaves + l: its final term; NaN where not written)."""
+        a, p, n = _idx(S)
+        nl, nit = len(x0[0]), len(x0)
+        kk = np.ascontiguousarray(np.array([int(x) for x in ks], dtype=np.uint64))
+        na = len(kk)
+        nd = max([len(m_) for m_ in list(evk_a) + [evkf_a] if m_ is not None] or [1])
+
+        def cst(cs):
+            return (C.c_void_p * (nl * na))(*[c_.h if c_ is not None else None for row in cs for c_ in row])
+
+        def keys(evk, cnt):
+            arr = (C.c_void_p * max(1, cnt * nd))()
+            for j, mat in enumerate(evk):
+                for i in range(nd):
+                    arr[j * nd + i] = mat[i].h if mat is not None else None
+            return arr
+        ex = np.ascontiguousarray(np.array([int(bool(e)) for e in ext], dtype=np.int32)) if ext is not None else None
+        bad = consts1 is not None
+        args = (_arr([x for it in x0 for x in it]), _arr([x for it in x1 for x in it]), nl, nit,
+                ex.ctypes.data_as(C.POINTER(C.c_int32)) if ex is not None else None, p, n, C.c_uint64(int(ptxt_space)),
+                na, kk.ctypes.data_as(u64p), keys(evk_a, na), keys(evk_b, na), cst(consts), cst(consts1) if bad else None,
+                C.c_uint64(int(kfinal)), keys([evkf_a], 1) if bad else None, keys([evkf_b], 1) if bad else None, nd,
+                _arr(acc0), _arr(acc1), int(bool(accumulate)))
+        if not norms:
+            self._ck(self.lib.hb_full_linear_map_leaves(*args))
+            return None
+        T = 2 * nl if bad else nl
+        out = np.full((nit, T, 10), np.nan, dtype=np.float64)
+        self._ck(self.lib.hb_full_linear_map_leaves_norm(*args, out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
+
     cls.automorph_keyswitch_digits = automorph_keyswitch_digits
     cls.hoisted_linear_map = hoisted_linear_map
     cls.bsgs_linear_map = bsgs_linear_map
     cls.block_linear_map = block_linear_map
+    cls.full_linear_map_leaves = full_linear_map_leaves
     return cls
 
 

@@ -296,6 +296,46 @@ int hb_block_linear_map_norm(hb_poly* const* digits, int maxdig, int nitems, con
                              hb_poly* const* consts, hb_poly* const* consts1, uint64_t kfinal,
                              hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
                              hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms);
+/* Full linear map leaves (SURVEY 8f-1): the last dimension of MatMulFullExec::rec_mul (src/matmul.cpp:2141-2148), every
+ * leaf a hoisted MatMul1DExec::mul (:1226-1252 native, :1253-1283 bad dimension), all leaves of a ciphertext summed into
+ * one accumulator.  Leaf l of item it is the two-part ciphertext (x0, x1)[it*nleaves + l]: over S | special when
+ * ext[l] != 0 (a rotated leaf, not cleaned), over S otherwise (ext == NULL: every leaf over S).  Amounts k[t] (t < namt)
+ * with matrices evk_a/evk_b (matrix t = entries t*ndig_evk .., ignored and may be NULL where k[t] == 1); constants
+ * consts[l*namt + t] over S | special (HElib's cache.multiplier of leaf l; NULL: a zero diagonal, skipped as MulAdd skips
+ * it).  consts1 != NULL selects a bad leaf dimension: consts1 has the layout of consts, kfinal is genToPow(dim, -D) with
+ * matrix evkf.  For every item, over S | special, in HElib's order of steps:
+ *   x_l <- cleanUp(x_l)      ext[l]: scaleDownToSet to S with ptxt_space (dropSmallAndSpecialPrimes)
+ *   D_l  = breakIntoDigits(x_l.part1) over S
+ *   r_{l,t} = BasicAutomorphPrecon(x_l).automorph(k[t])          (k[t] == 1: P*(c0, c1), addPrimesAndScale)
+ *   acc0/acc1 (+)= sum_l sum_t consts[l*namt + t] * r_{l,t}  [ + sum_l term( sum_t consts1[l*namt + t] * r_{l,t}, kfinal ) ]
+ * term(y, k) = y for k == 1, otherwise smartAutomorph(k) in the extended form of hb_bsgs_linear_map: sigma_k, the mod-down
+ * to S, breakIntoDigits over S and the key switch.  accumulate = 0 overwrites.  The items share amounts, matrices and
+ * constants; the inputs are read-only.  Power-of-two and general m; expanded or seeded evk_a.  Per chunk of at most 32
+ * (item, leaf) pairs: the chunk's mod-downs and digits run in one batched launch each; one k_ks_leafmap pass per group of
+ * at most 32 amounts sums every leaf's rotations into the accumulators (and the per-leaf sums of the bad dimension), its
+ * matrices (seeded: regenerated once per chunk and group of amounts) read once for the up to 4 leaves a thread holds; in a bad
+ * dimension sigma_kfinal, the mod-down, digits and k_ks_giant follow for the chunk's per-leaf sums.  The scratch is at most
+ * min(32, nitems*nleaves)*(bad ? 4 + ndig : 2 + ndig) + (bad and evkf_a seeded ? ndig : 0) polys whatever nleaves and
+ * namt are.  Errors, all reported before any launch: an amount not in Z_m^*, S not within the ctxt primes, or a seeded
+ * evk_a without a needed row -> HB_ERR_INDEX_SET; nleaves, nitems or namt <= 0, ext not 0/1, no amounts, too few matrix
+ * columns, S with more than 8 digits, a missing matrix, an accumulator aliasing an input or another accumulator, or a
+ * seeded handle other than in evk_a -> HB_ERR_BAD_ARG.  Stream-ordered, no synchronisation; after the first call, a call
+ * of the same shape allocates nothing. */
+int hb_full_linear_map_leaves(hb_poly* const* x0, hb_poly* const* x1, int nleaves, int nitems, const int32_t* ext,
+                              const int32_t* S, int nS, uint64_t ptxt_space, int namt, const uint64_t* k,
+                              hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* consts, hb_poly* const* consts1,
+                              uint64_t kfinal, hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                              hb_poly* const* acc0, hb_poly* const* acc1, int accumulate);
+/* The same, returning the norms the noise bookkeeping of the leaves needs, in the layout of hb_block_linear_map_norm: with
+ * T = nleaves (native) or 2*nleaves (bad dimension), norms[(item*T + e)*(8 + 2) + i].  Entry e = l is leaf l's cleanUp and
+ * hoisting: ln ||E_i|| of its digit i (i < ndig, breakIntoDigits' norms) and, for ext[l] != 0, at offsets 8 and 9 the
+ * ||delta/P|| of parts 0 and 1 of its mod-down (hb_scale_down_norm).  In the bad dimension entry nleaves + l is leaf l's
+ * final term (kfinal): its digits' and mod-down's norms likewise.  Entries not computed are not written.  Synchronises. */
+int hb_full_linear_map_leaves_norm(hb_poly* const* x0, hb_poly* const* x1, int nleaves, int nitems, const int32_t* ext,
+                                   const int32_t* S, int nS, uint64_t ptxt_space, int namt, const uint64_t* k,
+                                   hb_poly* const* evk_a, hb_poly* const* evk_b, hb_poly* const* consts, hb_poly* const* consts1,
+                                   uint64_t kfinal, hb_poly* const* evkf_a, hb_poly* const* evkf_b, int ndig_evk,
+                                   hb_poly* const* acc0, hb_poly* const* acc1, int accumulate, double* norms);
 /* Ctxt::tensorProduct of two canonical 2-part ciphertexts (src/Ctxt.cpp:1563-1608) */
 int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1,
               hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int nitems, const int32_t* idx, int n);

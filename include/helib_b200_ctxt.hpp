@@ -1410,6 +1410,263 @@ inline void BlockMatMul1D(Ctxt& ctxt, long gen, long D, long d, const std::vecto
   ctxt = out;
 }
 
+// ---- MatMulFullExec::mul (src/matmul.cpp:2132-2273) and MatMul1DExec::mul's hoisted branches (:1226-1283) ----------
+constexpr long kBsgsMulThresh = 50;   // HELIB_BSGS_MUL_THRESH (= HELIB_KEYSWITCH_THRESH): larger dimensions take BSGS
+// One dimension of a full-matrix map: its generator, order D and whether it is native.  A bad outer dimension also has the
+// masks getMask_zzX(dim, i) as constants with their sizes, masks[i] for 1 <= i < D (masks[0] is not used).
+struct FullDim { long gen; long D; bool native; std::vector<BsgsDiag> masks; };
+
+namespace detail {
+// MatMul1DExec::mul's hoisted branches transcribed (FULL strategy, one thread): cleanUp, then
+//   acc = sum_i cache[i] * automorph(gen^i)  (+ smartAutomorph(gen^-D) of sum_i cache1[i] * automorph(gen^i), bad)
+inline void matmul1dLoop(Ctxt& ctxt, long gen, long D, const std::vector<BsgsDiag>& cache, const std::vector<BsgsDiag>* cache1) {
+  const long m = ctxt.context.getM();
+  ctxt.cleanUp();
+  BasicAutomorphPrecon precon(ctxt);
+  Ctxt acc(ctxt.pubKey, ctxt.ptxtSpace), acc1(ctxt.pubKey, ctxt.ptxtSpace);
+  for (long i = 0; i < D; i++) {
+    const BsgsDiag& c = cache[(size_t)i];
+    const BsgsDiag* c1 = cache1 ? &(*cache1)[(size_t)i] : nullptr;
+    if (!c.c && !(c1 && c1->c)) continue;
+    std::shared_ptr<Ctxt> r = precon.automorph(genToPow(gen, i, m));
+    if (c.c) { Ctxt t(*r); BasicAutomorphPrecon::mulConst(t, c); acc += t; }
+    if (c1 && c1->c) { Ctxt t(*r); BasicAutomorphPrecon::mulConst(t, *c1); acc1 += t; }
+  }
+  if (cache1 && !acc1.isEmpty()) { acc1.smartAutomorph(genToPow(gen, -D, m)); acc += acc1; }
+  ctxt = acc;
+}
+// The metadata modDownToSet(S) gives a ciphertext over S | special, from the device's ||delta/P|| of its two parts
+// (nr[kNormStride8], nr[kNormStride8 + 1])
+inline void modDownMeta(Ctxt& t, const double* nr, const IndexSet& S) {
+  const XD addedNoise = XD(nr[kNormStride8]) + XD(nr[kNormStride8 + 1]) * XD::exp(std::log(t.pubKey.skBound));
+  const XD f = XD::exp(t.pubKey.logOfProduct(t.context.getSpecialPrimes()));
+  t.ratFactor = t.ratFactor / f;
+  t.noiseBound = t.noiseBound / f;
+  t.noiseBound = t.noiseBound + addedNoise;
+  t.primeSet = S;
+}
+// sum_l MatMul1DExec::mul(leaves[l]) for leaves of one hoisted dimension (D <= kBsgsMulThresh), the cache of leaf l at
+// cache[l] (cache1[l] for a bad dimension): one hb_full_linear_map_leaves_norm call, and the loop's metadata replayed term
+// by term, leaf by leaf, from the norms it returns.  Returns false, with out untouched, where one call cannot reproduce the
+// loop: CKKS, a leaf that is not 2-part canonical under the first leaf's key or whose cleanUp would not land on the common
+// set S, an amount without a direct matrix, sums that would not be a plain add, or a result not over S | special.
+inline bool leavesFused(Ctxt& out, const std::vector<const Ctxt*>& leaves, long gen, long D,
+                        const std::vector<const std::vector<BsgsDiag>*>& cache, const std::vector<const std::vector<BsgsDiag>*>& cache1) {
+  using P = BasicAutomorphPrecon;
+  if (leaves.empty() || D > kBsgsMulThresh) return false;
+  const Ctxt& c0 = *leaves[0];
+  if (c0.isCKKS()) return false;
+  const Context& context = c0.context;
+  const KeyInfo& pubKey = c0.pubKey;
+  const long m = context.getM();
+  const bool bad = !cache1.empty();
+  const long keyID = c0.getKeyID();
+  const IndexSet special = context.getSpecialPrimes();
+  const IndexSet S = c0.primeSet / special;
+  const IndexSet full = S | special;
+  if (empty(S) || !(S <= context.getCtxtPrimes()) || !S.disjointFrom(context.getSmallPrimes())) return false;
+  const long nl = (long)leaves.size();
+  std::vector<int32_t> ext((size_t)nl);
+  for (long l = 0; l < nl; l++) {
+    const Ctxt& x = *leaves[(size_t)l];
+    if (&x.pubKey != &pubKey || x.ptxtSpace != c0.ptxtSpace || x.parts.size() != 2 || x.getPartIndexByHandle(SKHandle()) < 0 ||
+        x.getPartIndexByHandle(SKHandle(1, 1, keyID)) < 0 || !(x.primeSet == S || x.primeSet == full))
+      return false;
+    ext[(size_t)l] = x.primeSet == full;
+  }
+  long nd = 0;   // the digits of S (src/DoubleCRT.cpp:485-493)
+  for (IndexSet rem = S; !empty(rem) && nd < (long)context.getDigits().size(); nd++) rem.remove(context.getDigit(nd));
+  bool ok = true;
+  auto direct = [&](long k) -> const KeySwitch* {
+    if (k == 1) return nullptr;
+    if (!pubKey.isReachable(k, keyID)) { ok = false; return nullptr; }
+    const KeySwitch* w = pubKey.getNextKSWmatrix(k, keyID);
+    if (w->fromKey.powerOfX != k || w->toKeyID != keyID || (long)w->b.size() < nd) ok = false;
+    return w;
+  };
+  std::vector<long> k((size_t)D);
+  std::vector<const KeySwitch*> W((size_t)D);
+  for (long t = 0; t < D; t++) { k[(size_t)t] = genToPow(gen, t, m); W[(size_t)t] = direct(k[(size_t)t]); }
+  const long kf = genToPow(gen, -D, m);
+  const KeySwitch* Wf = bad ? direct(kf) : nullptr;
+  if (!ok) return false;
+  // ---- the call
+  std::vector<hb_poly*> x0((size_t)nl), x1((size_t)nl), cs((size_t)(nl * D), nullptr), cs1(bad ? (size_t)(nl * D) : 0, nullptr);
+  std::vector<hb_poly*> ea((size_t)(D * nd), nullptr), eb((size_t)(D * nd), nullptr), efa((size_t)nd, nullptr), efb((size_t)nd, nullptr);
+  for (long l = 0; l < nl; l++) {
+    const Ctxt& x = *leaves[(size_t)l];
+    x0[(size_t)l] = x.parts[(size_t)x.getPartIndexByHandle(SKHandle())].dcrt.handle();
+    x1[(size_t)l] = x.parts[(size_t)x.getPartIndexByHandle(SKHandle(1, 1, keyID))].dcrt.handle();
+    for (long t = 0; t < D; t++) {
+      if ((*cache[(size_t)l])[(size_t)t].c) cs[(size_t)(l * D + t)] = (*cache[(size_t)l])[(size_t)t].c->handle();
+      if (bad && (*cache1[(size_t)l])[(size_t)t].c) cs1[(size_t)(l * D + t)] = (*cache1[(size_t)l])[(size_t)t].c->handle();
+    }
+  }
+  auto keys = [&](const KeySwitch* w, hb_poly** a, hb_poly** b) { if (w) for (long i = 0; i < nd; i++) { a[i] = w->aHandle((size_t)i); b[i] = w->b[(size_t)i].handle(); } };
+  for (long t = 0; t < D; t++) keys(W[(size_t)t], &ea[(size_t)(t * nd)], &eb[(size_t)(t * nd)]);
+  keys(Wf, efa.data(), efb.data());
+  std::vector<uint64_t> ku(k.begin(), k.end());
+  const long T = bad ? 2 * nl : nl;
+  std::vector<double> norms((size_t)T * (kNormStride8 + 2), 0.0);
+  DoubleCRT a0(context, full), a1(context, full);
+  {
+    hb_poly* o0[1] = {a0.handle()}; hb_poly* o1[1] = {a1.handle()};
+    auto Sv = S.vec();
+    check(hb_full_linear_map_leaves_norm(x0.data(), x1.data(), (int)nl, 1, ext.data(), Sv.data(), (int)Sv.size(), (uint64_t)c0.ptxtSpace,
+                                         (int)D, ku.data(), ea.data(), eb.data(), cs.data(), bad ? cs1.data() : nullptr, (uint64_t)kf,
+                                         efa.data(), efb.data(), (int)nd, o0, o1, 0, norms.data()));
+  }
+  // ---- metadata: the loop's, leaf by leaf and term by term in its order
+  auto meta_of = [&](const Ctxt& c) {
+    Ctxt t(pubKey, c.ptxtSpace);
+    t.primeSet = c.primeSet; t.noiseBound = c.noiseBound; t.intFactor = c.intFactor; t.ratFactor = c.ratFactor; t.ptxtMag = c.ptxtMag;
+    return t;
+  };
+  auto plain = [&](const Ctxt& a, const Ctxt& b) {   // a += b must be a plain add
+    Ctxt x = a, y = b;
+    P::modUpMeta(x, b.primeSet); P::modUpMeta(y, a.primeSet);
+    return x.ptxtSpace == y.ptxtSpace && x.intFactor == y.intFactor;
+  };
+  XD max_ks_noise(0.0);
+  for (const KeySwitch& ks : pubKey.keySwitching) if (max_ks_noise < ks.noiseBound) max_ks_noise = ks.noiseBound;
+  const double logP = pubKey.logOfProduct(special);
+  Ctxt meta(pubKey, c0.ptxtSpace);
+  bool first = true;
+  for (long l = 0; l < nl; l++) {
+    const double* nr = &norms[(size_t)l * (kNormStride8 + 2)];
+    Ctxt cl = meta_of(*leaves[(size_t)l]);   // cleanUp
+    if (ext[(size_t)l]) modDownMeta(cl, nr, S);
+    XD addedNoise(0.0);                        // BasicAutomorphPrecon's hoisting noise
+    for (long i = 0; i < nd; i++) addedNoise = addedNoise + XD::exp(nr[i]);
+    addedNoise = addedNoise * max_ks_noise;
+    XD hn = cl.noiseBound * XD::exp(logP);
+    hn = hn + addedNoise;
+    Ctxt sums[2] = {Ctxt(pubKey, cl.ptxtSpace), Ctxt(pubKey, cl.ptxtSpace)};
+    bool firsts[2] = {true, true};
+    for (long t = 0; t < D; t++)
+      for (int set = 0; set < (bad ? 2 : 1); set++) {
+        const BsgsDiag& c = (*(set ? cache1 : cache)[(size_t)l])[(size_t)t];
+        if (!c.c) continue;
+        Ctxt r = meta_of(cl);
+        if (k[(size_t)t] != 1) { r = Ctxt(pubKey, cl.ptxtSpace); r.noiseBound = hn; r.intFactor = cl.intFactor; r.primeSet = full; }
+        P::mulConstMeta(r, c);
+        if (!firsts[set] && !plain(sums[set], r)) return false;
+        P::addMeta(sums[set], firsts[set], r);
+      }
+    if (bad && !firsts[1]) {
+      Ctxt t = sums[1];
+      if (Wf) {
+        if (!(t.primeSet == full)) return false;
+        relinTermMeta(t, &norms[(size_t)(nl + l) * (kNormStride8 + 2)], true, *Wf, nd, S);
+      }
+      if (!firsts[0] && !plain(sums[0], t)) return false;
+      P::addMeta(sums[0], firsts[0], t);
+    }
+    if (firsts[0]) continue;   // an empty leaf: acc += 0 changes nothing
+    if (!first && !plain(meta, sums[0])) return false;
+    P::addMeta(meta, first, sums[0]);
+  }
+  if (first || !(meta.primeSet == full)) return false;
+  Ctxt res(pubKey, meta.ptxtSpace);
+  res.primeSet = meta.primeSet; res.noiseBound = meta.noiseBound; res.intFactor = meta.intFactor;
+  res.ratFactor = meta.ratFactor; res.ptxtMag = meta.ptxtMag;
+  res.parts.emplace_back(a0, SKHandle());
+  res.parts.emplace_back(a1, SKHandle(1, 1, keyID));
+  out = res;
+  return true;
+}
+}  // namespace detail
+
+// MatMul1DExec::mul's hoisted branches (FULL strategy, one thread; src/matmul.cpp:1226-1283): ctxt becomes
+// sum_i cache[i] * rot_{gen^i}(ctxt) (+ smartAutomorph(gen^-D) of sum_i cache1[i] * rot_{gen^i}(ctxt) for a bad dimension,
+// cache1 non-empty).  The native branch is BasicAutomorphPrecon::linearCombination; the bad branch is one
+// hb_full_linear_map_leaves_norm call with a single leaf, with the loop's bits and metadata, or the transcribed loop where
+// one call cannot reproduce it.  D > kBsgsMulThresh takes HElib's BSGS branch, hb::MatMul1DBSGS.  BGV only.
+inline void MatMul1D(Ctxt& ctxt, long gen, long D, const std::vector<BsgsDiag>& cache, const std::vector<BsgsDiag>& cache1 = {}) {
+  if (ctxt.isCKKS()) throw LogicError("hb::MatMul1D: BGV only (CKKS takes linearCombinationCKKS or MatMul1DBSGS)");
+  if (D <= 0 || (long)cache.size() != D || (!cache1.empty() && (long)cache1.size() != D)) throw InvalidArgument("MatMul1D: one diagonal per index");
+  if (D > kBsgsMulThresh) { ctxt.cleanUp(); MatMul1DBSGS(ctxt, gen, D, cache, cache1); return; }
+  const long m = ctxt.context.getM();
+  ctxt.cleanUp();
+  if (cache1.empty()) {
+    std::vector<long> k; std::vector<const DoubleCRT*> cs; std::vector<double> sz;
+    for (long i = 0; i < D; i++) if (cache[(size_t)i].c) { k.push_back(genToPow(gen, i, m)); cs.push_back(cache[(size_t)i].c); sz.push_back(cache[(size_t)i].size); }
+    if (k.empty()) { ctxt = Ctxt(ctxt.pubKey, ctxt.ptxtSpace); return; }
+    ctxt = *BasicAutomorphPrecon(ctxt).linearCombination(k, cs, sz);
+    return;
+  }
+  Ctxt out(ctxt.pubKey, ctxt.ptxtSpace);
+  if (detail::leavesFused(out, {&ctxt}, gen, D, {&cache}, {&cache1})) { ctxt = out; return; }
+  detail::matmul1dLoop(ctxt, gen, D, cache, &cache1);
+}
+
+// MatMulFullExec::mul (src/matmul.cpp:2132-2273, BGV; FULL key strategy in every dimension, one thread): cleanUp, then
+// rec_mul over the dimensions sorted as MatMulDimComp sorts them (smaller order first, native before bad on ties).  The
+// outer levels run as rec_mul does, with BasicAutomorphPrecon rotations (hb_automorph_keyswitch_digits) and, for a bad
+// outer dimension, tmp*mask + tmp1 - tmp1*mask with tmp1 rotated from smartAutomorph(gen^-D).  leaves[idx] (leaves1[idx]
+// for a bad last dimension) is the cache of leaf idx in rec_mul's order, one diagonal per index of the last dimension.
+// The leaves then go through one hb_full_linear_map_leaves_norm call (hb::detail::leavesFused, shared with hb::MatMul1D),
+// so the result has the transcribed loop's bits and metadata; the transcribed leaves run instead where that call cannot
+// reproduce them, and a last dimension above kBsgsMulThresh takes hb::MatMul1DBSGS per leaf, as HElib's BSGS branch.
+// CKKS: LogicError, as HElib (HELIB_NO_CKKS_IMPL).
+inline void MatMulFull(Ctxt& ctxt, std::vector<FullDim> dims, const std::vector<std::vector<BsgsDiag>>& leaves,
+                       const std::vector<std::vector<BsgsDiag>>& leaves1 = {}) {
+  if (ctxt.isCKKS()) throw LogicError("MatMulFullExec: not implemented for CKKS");
+  if (dims.empty()) throw InvalidArgument("MatMulFull: no dimensions");
+  std::stable_sort(dims.begin(), dims.end(), [](const FullDim& a, const FullDim& b) { return a.D < b.D || (a.D == b.D && a.native && !b.native); });
+  size_t nl = 1;
+  for (size_t i = 0; i + 1 < dims.size(); i++) {
+    nl *= (size_t)dims[i].D;
+    if (!dims[i].native && (long)dims[i].masks.size() != dims[i].D) throw InvalidArgument("MatMulFull: a bad dimension needs D masks");
+  }
+  const FullDim& last = dims.back();
+  if (leaves.size() != nl || (!last.native && leaves1.size() != nl) || (last.native && !leaves1.empty())) throw InvalidArgument("MatMulFull: one cache per leaf");
+  for (size_t l = 0; l < nl; l++)
+    if ((long)leaves[l].size() != last.D || (!last.native && (long)leaves1[l].size() != last.D)) throw InvalidArgument("MatMulFull: one diagonal per index");
+  const long m = ctxt.context.getM();
+  ctxt.cleanUp();
+  // the outer levels of rec_mul; the leaf inputs in its order
+  std::vector<Ctxt> L;
+  L.reserve(nl);
+  std::function<void(const Ctxt&, size_t)> rec = [&](const Ctxt& c, size_t di) {
+    if (di + 1 == dims.size()) { L.push_back(c); return; }
+    const FullDim& d = dims[di];
+    if (d.native) {
+      BasicAutomorphPrecon precon(c);
+      for (long i = 0; i < d.D; i++) rec(*precon.automorph(genToPow(d.gen, i, m)), di + 1);
+      return;
+    }
+    Ctxt c1(c);
+    c1.smartAutomorph(genToPow(d.gen, -d.D, m));
+    BasicAutomorphPrecon precon(c), precon1(c1);
+    for (long i = 0; i < d.D; i++) {
+      if (i == 0) { rec(c, di + 1); continue; }
+      std::shared_ptr<Ctxt> tmp = precon.automorph(genToPow(d.gen, i, m)), tmp1 = precon1.automorph(genToPow(d.gen, i, m));
+      const BsgsDiag& mk = d.masks[(size_t)i];
+      tmp->multByConstant(*mk.c, mk.size);
+      *tmp += *tmp1;
+      tmp1->multByConstant(*mk.c, mk.size);
+      tmp->addCtxt(*tmp1, /*negative=*/true);
+      rec(*tmp, di + 1);
+    }
+  };
+  rec(ctxt, 0);
+  // the leaves
+  Ctxt acc(ctxt.pubKey, ctxt.ptxtSpace);
+  if (last.D <= kBsgsMulThresh) {
+    std::vector<const Ctxt*> lp; std::vector<const std::vector<BsgsDiag>*> cp, cp1;
+    for (size_t l = 0; l < nl; l++) { lp.push_back(&L[l]); cp.push_back(&leaves[l]); if (!last.native) cp1.push_back(&leaves1[l]); }
+    if (detail::leavesFused(acc, lp, last.gen, last.D, cp, cp1)) { ctxt = acc; return; }
+  }
+  for (size_t l = 0; l < nl; l++) {   // transforms[idx].mul(tmp); acc += tmp
+    Ctxt tmp(L[l]);
+    if (last.D > kBsgsMulThresh) { tmp.cleanUp(); MatMul1DBSGS(tmp, last.gen, last.D, leaves[l], last.native ? std::vector<BsgsDiag>{} : leaves1[l]); }
+    else detail::matmul1dLoop(tmp, last.gen, last.D, leaves[l], last.native ? nullptr : &leaves1[l]);
+    acc += tmp;
+  }
+  ctxt = acc;
+}
+
 // ---- SURVEY 8f-2: the steps either side of the path ------------------------------------------------------------
 // Sampling follows the reference's DISTRIBUTIONS (src/sample.cpp); its bit stream (NTL's PRG) is not restated, so
 // the sampled values are an input of Encrypt below and "parity unpinned" is confined to them.
