@@ -488,7 +488,9 @@ __device__ __forceinline__ i64 hb_conv_v(const HbConvDev* cv, const u64* y, int 
   const u64 margin = 4ULL * (u64)n;
   int sign = 2;  // unknown
   if (F >= 0 - margin) {  // could round up once the truncation error is added back: decide exactly
-    v = hb_crt_exact(cv, y, ystride, &sign, nullptr, 0, 0);
+    const i64 ve = hb_crt_exact(cv, y, ystride, &sign, nullptr, 0, 0);
+    if (ve != v) F = 0;   // rounded up: x/Q is -1/2 (within the margin), not the +1/2 the truncated F reads
+    v = ve;
     if (stats) atomicAdd(stats, 1ULL);
   }
   if (bgv && cv->has_p) {

@@ -579,10 +579,11 @@ def _engine_hoist(cls):
                                                 _arr(acc0), _arr(acc1), int(bool(accumulate))))
 
     def bsgs_linear_map(self, baby0, baby1, S, ks, consts, evk_a, evk_b, acc0, acc1, extended=False, ptxt_space=1,
-                        scal=None, accumulate=False):
+                        scal=None, accumulate=False, norms=False):
         """acc (+)= the giant steps of a BSGS linear map over S | special, for every item (hb_bsgs_linear_map).
         baby0 / baby1: per item, the list of the baby steps' parts; consts: per giant step, one Poly (or None) per baby
-        step; ks: the giant amounts; evk_a / evk_b: per giant step, the list of matrix Polys (None where k == 1)."""
+        step; ks: the giant amounts; evk_a / evk_b: per giant step, the list of matrix Polys (None where k == 1).
+        norms=True calls hb_bsgs_linear_map_norm and returns its norms as [item][giant step][10] (NaN where not written)."""
         a, p, n = _idx(S)
         nb = len(baby0[0])
         kk = np.ascontiguousarray(np.array([int(x) for x in ks], dtype=np.uint64))
@@ -597,10 +598,16 @@ def _engine_hoist(cls):
                     arr[j * nd + i] = mat[i].h if mat is not None else None
             return arr
         sc = np.ascontiguousarray(np.array([int(x) for x in scal], dtype=np.uint64)) if scal is not None else None
-        self._ck(self.lib.hb_bsgs_linear_map(_arr([x for it in baby0 for x in it]), _arr([x for it in baby1 for x in it]), nb, len(baby0),
-                                             p, n, int(bool(extended)), C.c_uint64(int(ptxt_space)), ng, kk.ctypes.data_as(u64p), cs,
-                                             sc.ctypes.data_as(u64p) if sc is not None else None, keys(evk_a), keys(evk_b), nd,
-                                             _arr(acc0), _arr(acc1), int(bool(accumulate))))
+        args = (_arr([x for it in baby0 for x in it]), _arr([x for it in baby1 for x in it]), nb, len(baby0),
+                p, n, int(bool(extended)), C.c_uint64(int(ptxt_space)), ng, kk.ctypes.data_as(u64p), cs,
+                sc.ctypes.data_as(u64p) if sc is not None else None, keys(evk_a), keys(evk_b), nd,
+                _arr(acc0), _arr(acc1), int(bool(accumulate)))
+        if not norms:
+            self._ck(self.lib.hb_bsgs_linear_map(*args))
+            return None
+        out = np.full((len(baby0), ng, 10), np.nan, dtype=np.float64)
+        self._ck(self.lib.hb_bsgs_linear_map_norm(*args, out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out
 
     def block_linear_map(self, digits, S, c0, c1, k0, evk0_a, evk0_b, k1, evk1_a, evk1_b, consts, acc0, acc1,
                          consts1=None, kfinal=1, evkf_a=None, evkf_b=None, ptxt_space=1, accumulate=False, norms=False):
