@@ -214,6 +214,7 @@ struct HbCrtJob {            // DoubleCRT::toPoly: exact balanced integer per co
   const u64* src;            // coefficient-form rows (after full inverse transform incl. N^-1 ... see k_crt)
   u64* out;                  // [N][Lout] two's complement limbs
   u64 factor, factor_s;      // k_crt_modp: result multiplier mod p (+Shoup wrt p)
+  u64* stats;                // k_crt_modp: [0] += number of exact-fallback evaluations
 };
 
 enum {
@@ -610,7 +611,7 @@ __global__ void __launch_bounds__(HB_THREADS) k_crt_modp(const HbPrimeDev* __res
     int pi = cv->src_prime[j];
     y[j] = hb_mul_shoup(J.src[(size_t)pi * J.N + k], tabs.t[j], tabs.t_s[j], primes[pi].q);
   }
-  const i64 v = hb_conv_v(cv, y, 1, nullptr, nullptr, false);
+  const i64 v = hb_conv_v(cv, y, 1, J.stats, nullptr, false);
   u64 hi = 0, lo = 0;
   for (int j = 0; j < n; j++) hb_mac128(hi, lo, y[j], cv->cp[j]);
   hb_mac128(hi, lo, (u64)v, cv->negQ_p);

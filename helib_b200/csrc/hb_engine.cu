@@ -1744,7 +1744,7 @@ extern "C" int hb_to_poly_mod_p(hb_poly* p, const int32_t* idx, int n, uint64_t 
   u64* d_out; size_t bytes = c->N * sizeof(u64);
   HB_CUDA(cudaMalloc((void**)&d_out, bytes));
   HbCrtJob J; memset(&J, 0, sizeof(J));
-  J.cv = E->d; J.N = (int)c->N; J.src = coef; J.out = d_out; J.factor = factor; J.factor_s = h_shoup(factor, ptxt_space);
+  J.cv = E->d; J.N = (int)c->N; J.src = coef; J.out = d_out; J.factor = factor; J.factor_s = h_shoup(factor, ptxt_space); J.stats = c->d_stats;
   HbCrtTabs T; T.t = E->d_t; T.t_s = E->d_t_s;
   dim3 grid((unsigned)((c->N + HB_THREADS - 1) / HB_THREADS));
   pre_launch(c);
