@@ -457,6 +457,112 @@ __global__ void __launch_bounds__(256, 1) k1_fwd_blk_tensor(const HbPrimeDev* __
   hb1_cp_wait<0>();
 }
 
+// The squaring counterpart of k1_fwd_blk_tensor: the rescale of one ciphertext's two parts and its self-tensor in one
+// forward blk pass (bringToSet(naturalPrimeSet()) of a0, a1, then Ctxt::tensorProduct(*this, *this), src/Ctxt.cpp:1704-1708,
+// 1563-1608).  src[2*it + k] is the coefficient-side tile of part k left by the conversion, dst[2*it + k] that part's rows,
+// dst2[it] the s^2 output.  A unit (row, group of 16 blocks, item) runs the forward blk phase of a0 and a1 in turn with the
+// twiddles loaded once, applies the subscale epilogue (v = (old - x) * P^-1, lazy in [0,4q)) and stores, canonical,
+//   a0 <- a0'^2,   a1 <- 2*a0'*a1',   o2 <- a1'^2
+// (2*a0'*a1' is the 128-bit sum a0'*a1' + a0'*a1', below 2^125, reduced once, as k1_fwd_blk_tensor reduces a0'*b1' + a1'*b0').
+// a0' waits for part 1 in one per-thread slot array V of shared memory.  Part 0's old values are read before anything is
+// stored: all three outputs go out with part 1, after its own old values have landed.
+// smem: S[2][HB1_STAGE] | O[16][256] | TW1[256] | V[16][256]
+template <bool SP>
+__global__ void __launch_bounds__(256, 1) k1_fwd_blk_square(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT Hb1BlkJob J) {
+  HB_SMEM_DECL
+  u64* S = HB_SMEM;
+  u64* O = S + 2 * HB1_STAGE;
+  ulonglong2* TW1 = (ulonglong2*)(O + 16 * 256);
+  u64* V = (u64*)(TW1 + 256);
+  const int tid = threadIdx.x;
+  const int n1 = J.logN - 8;
+  const int G = 1 << (n1 - 4);
+  const long U = (long)J.rows.n * G * J.nitems;
+  const long ubeg = U * blockIdx.x / gridDim.x, uend = U * (blockIdx.x + 1) / gridDim.x;
+  if (ubeg >= uend) return;
+  const int blk1 = tid >> 4, lo = tid & 15;
+  const int hi = tid >> 4, blk2 = tid & 15;
+  const unsigned hrev = hb1_brev4(hi);
+  const int own = blk1 * HB1_BS + lo;   // + HB1_RS * r
+  u64* const Vt = V + tid;              // a0' of position l: Vt[l * 256]
+  Hb1TwPtr tw1;
+  tw1.p[0] = TW1 + blk1 * 16; tw1.p[1] = tw1.p[0] + 1; tw1.p[2] = tw1.p[0] + 3; tw1.p[3] = tw1.p[0] + 7;
+
+  auto prefetch = [&](u64* Sn, const Hb1Unit& x, int k) {
+    const unsigned b = hb_brev((x.ug << 4) + blk1, n1);
+    const u64* src = J.src[2 * x.it + k] + ((size_t)J.rows.prime[x.rowi] << J.logN) + ((size_t)b << 8) + lo;
+    hb1_unroll<16>([&](auto r) { hb1_cp8(Sn + own + HB1_RS * r, src + 16 * r); });
+  };
+  Hb1Unit cur = hb1_unit(ubeg, G, J.nitems);
+  prefetch(S, cur, 0);
+  hb1_cp_commit();
+  int key = -1;
+  u64 q = 0, sc = 0, sc_s = 0, c64 = 0, c64_s = 0, one_s = 0;
+  Hb1Mod M; M.nq = 0; M.qb = 0; M.qb2 = 0; M.qt = 0; M.qsh = 0;
+  Hb1TwReg tw2;
+  for (long u = ubeg; u < uend; u++) {
+    if (cur.rowi * G + cur.ug != key) {   // new (row, block group): reload modulus and twiddles
+      key = cur.rowi * G + cur.ug;
+      const HbPrimeDev P = primes[J.rows.prime[cur.rowi]];
+      q = P.q; M.nq = P.nq; M.qb = P.qb; M.qb2 = P.qb + P.qb; M.qt = P.qt; M.qsh = P.qsh;
+      c64 = P.c64; c64_s = P.c64_s; one_s = P.one_s;
+      sc = J.scal[cur.rowi]; sc_s = J.scal_s[cur.rowi];
+      const unsigned b1 = hb_brev((cur.ug << 4) + blk1, n1), b2 = hb_brev((cur.ug << 4) + blk2, n1);
+      if (lo < 15) {  // entry e = (1<<k)-1+g of block blk1
+        int e = lo, k = e >= 7 ? 3 : (e >= 3 ? 2 : (e >= 1 ? 1 : 0));
+        int g = e - ((1 << k) - 1);
+        TW1[blk1 * 16 + e] = P.fw[((size_t)1 << (n1 + k)) + ((size_t)b1 << k) + g];
+      }
+      tw2.load([&](int k, int g) { return P.fw[((size_t)1 << (n1 + 4 + k)) + ((size_t)b2 << (4 + k)) + ((size_t)hi << k) + g]; });
+      __syncthreads();  // TW1 visible (the previous unit's trailing barrier ordered its last use)
+    }
+    const size_t doff = ((size_t)J.rows.prime[cur.rowi] << J.logN) + (cur.ug << 4) + blk2;
+    u64* const* dst = J.dst + 2 * cur.it;
+    u64* const o2 = J.dst2[cur.it];
+    const bool more = u + 1 < uend;
+    const Hb1Unit nxt = more ? hb1_unit_next(cur, G, J.nitems) : cur;
+#pragma unroll 1
+    for (int k = 0; k < 2; k++) {
+      u64* Sb = S + k * HB1_STAGE;
+      const u64* old = dst[k] + doff;
+      hb1_unroll<16>([&](auto l) { hb1_cp8(O + l * 256 + tid, old + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1)); });
+      hb1_cp_commit();
+      if (k == 0) prefetch(S + HB1_STAGE, cur, 1);
+      else if (more) prefetch(S, nxt, 0);
+      hb1_cp_commit();
+      hb1_cp_wait<2>();   // this part's inputs have landed (issued one part ago)
+      u64 a[16];
+      hb1_unroll<16>([&](auto r) { a[r] = Sb[own + HB1_RS * r]; });
+      hb1_r16_fwd<SP>(a, tw1, M);
+      hb1_unroll<16>([&](auto r) { Sb[own + HB1_RS * r] = a[r]; });
+      __syncthreads();
+      hb1_unroll<16>([&](auto l) { a[l] = Sb[blk2 * HB1_BS + HB1_RS * hi + l]; });
+      hb1_r16_fwd<SP>(a, tw2, M);
+      hb1_cp_wait<1>();   // old values of this part have landed
+      hb1_unroll<16>([&](auto l) {   // (old - x) * P^-1 in [0,4q), x in [0, 8q + 2^32), old < 4q
+        a[l] = hb1_shoup4<SP>(O[l * 256 + tid] - a[l] + (M.qb2 + M.qb), sc, sc_s, M);
+      });
+      if (k == 0) {   // a0'
+        hb1_unroll<16>([&](auto l) { Vt[l * 256] = a[l]; });
+      } else {        // a1': a0'^2, 2*a0'*a1', a1'^2 out
+        hb1_unroll<16>([&](auto l) {
+          const size_t o = doff + ((size_t)((hb1_brev4(l) << 4) | hrev) << n1);
+          const u64 x0 = Vt[l * 256], v = a[l];
+          u64 h = 0, w = 0;
+          hb1_mac128(h, w, x0, v);
+          hb1_mac128(h, w, x0, v);
+          dst[0][o] = hb_reduce128(__umul64hi(x0, x0), x0 * x0, q, c64, c64_s, one_s);
+          dst[1][o] = hb_reduce128(h, w, q, c64, c64_s, one_s);
+          o2[o] = hb_reduce128(__umul64hi(v, v), v * v, q, c64, c64_s, one_s);
+        });
+      }
+      __syncthreads();   // exchange reads of Sb / TW1 done before they are overwritten
+    }
+    cur = nxt;
+  }
+  hb1_cp_wait<0>();
+}
+
 // Inverse "blk" phase (bit-reversal + first 8 GS stages), same decomposition and pipelining.
 // smem: S[2][HB1_STAGE] | TW1[256]
 template <bool SP>

@@ -27,6 +27,9 @@ typedef unsigned __int128 u128;
 static size_t blk_tensor_smem() {   // k1_fwd_blk_tensor: S[2][HB1_STAGE] | O[16][256] | TW1[256] | V[3][16][256]
   return (2 * HB1_STAGE + 16 * 256 + 3 * 16 * 256) * sizeof(u64) + 256 * sizeof(ulonglong2);
 }
+static size_t blk_square_smem() {   // k1_fwd_blk_square: S[2][HB1_STAGE] | O[16][256] | TW1[256] | V[16][256]
+  return (2 * HB1_STAGE + 16 * 256 + 16 * 256) * sizeof(u64) + 256 * sizeof(ulonglong2);
+}
 
 // ------------------------------------------------------------------------------------------
 // errors
@@ -339,6 +342,8 @@ static int ctx_build(hb_ctx* c, hb_ctx** out, int device, uint64_t m, int nprime
   HB_CUDA(cudaFuncSetAttribute(k1_inv_blk<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
   HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk_tensor<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blk_tensor_smem()));
   HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk_tensor<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blk_tensor_smem()));
+  HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk_square<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blk_square_smem()));
+  HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk_square<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)blk_square_smem()));
 #endif
   *out = c;
   return HB_OK;
@@ -877,6 +882,29 @@ static int launch_blk_tensor_v1(hb_ctx* c, const u64* const* src, u64* const* ds
     if (all_special(c)) HB_LAUNCH(k1_fwd_blk_tensor<true>, grid, dim3(256), blk_tensor_smem(), c->stream, c->d_primes, J);
     else HB_LAUNCH(k1_fwd_blk_tensor<false>, grid, dim3(256), blk_tensor_smem(), c->stream, c->d_primes, J);
     HB_TRY(post_launch(c, "k1_fwd_blk_tensor", (u64)12 * nr * nitems * c->N * 8));   // 4 tiles + 4 old rows read, 4 rows written
+  }
+  return HB_OK;
+}
+// the rescale of nitems ciphertexts (src / dst: 2 per item, a0 a1) fused with their self-tensor into (a0, a1, o2):
+// k1_fwd_blk_square
+static int launch_blk_square_v1(hb_ctx* c, const u64* const* src, u64* const* dst, u64* const* o2, int nitems, const int32_t* idx, int n,
+                                const u64* scal) {
+  const int n1 = c->logN - 8;
+  for (int r0 = 0; r0 < n; r0 += HB_MAXROWS) {
+    int nr = std::min(HB_MAXROWS, n - r0);
+    Hb1BlkJob J; memset(&J, 0, sizeof(J));
+    J.logN = c->logN; J.epi = 1; J.lazy = 1;
+    fill_rows(J.rows, idx + r0, nr);
+    for (int i = 0; i < nr; i++) { J.scal[i] = scal[r0 + i]; J.scal_s[i] = h_shoup(scal[r0 + i], c->q[idx[r0 + i]]); }
+    J.nitems = nitems;
+    for (int i = 0; i < 2 * nitems; i++) { J.src[i] = src[i]; J.dst[i] = dst[i]; }
+    for (int i = 0; i < nitems; i++) J.dst2[i] = o2[i];
+    long units = (long)nr * nitems << (n1 - 4);
+    dim3 grid((unsigned)std::min<long>(units, std::max(1, c->resident_ctas / 2)));   // persistent CTAs, one per SM
+    pre_launch(c);
+    if (all_special(c)) HB_LAUNCH(k1_fwd_blk_square<true>, grid, dim3(256), blk_square_smem(), c->stream, c->d_primes, J);
+    else HB_LAUNCH(k1_fwd_blk_square<false>, grid, dim3(256), blk_square_smem(), c->stream, c->d_primes, J);
+    HB_TRY(post_launch(c, "k1_fwd_blk_square", (u64)7 * nr * nitems * c->N * 8));   // 2 tiles + 2 old rows read, 3 rows written
   }
   return HB_OK;
 }
@@ -3284,6 +3312,11 @@ extern "C" int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_p
   hb_ctx* c = nullptr;
   HB_TRY(check_polys(a0, nitems, &c, "hb_mul_relin_moddown")); HB_TRY(check_polys(a1, nitems, &c, "hb_mul_relin_moddown"));
   HB_TRY(check_polys(b0, nitems, &c, "hb_mul_relin_moddown")); HB_TRY(check_polys(b1, nitems, &c, "hb_mul_relin_moddown"));
+  {   // the product is formed in place over four distinct polys: a repeated one would receive two results
+    std::set<const hb_poly*> ops(a0, a0 + nitems); ops.insert(a1, a1 + nitems); ops.insert(b0, b0 + nitems); ops.insert(b1, b1 + nitems);
+    if (ops.size() != 4 * (size_t)nitems)
+      return hb_fail(HB_ERR_BAD_ARG, "hb_mul_relin_moddown: the operand polys must be distinct (to square a ciphertext, use hb_square_relin_moddown)");
+  }
   // bringToSet(common) on both operands: modDownToSet -> scaleDownToSet per part (src/Ctxt.cpp:393-562)
   for (int i = 0; i < nS; i++)
     if (std::find(S_in, S_in + nS_in, S[i]) == S_in + nS_in)
@@ -3356,6 +3389,110 @@ extern "C" int hb_inner_product(hb_poly* const* a0, hb_poly* const* a1, hb_poly*
     // modDownToSet(S) of the result, as hb_mul_relin_moddown ends (src/Ctxt.cpp:589-593)
     two.clear();
     for (int i = 0; i < nit; i++) { two.push_back(out0[i0 + i]); two.push_back(out1[i0 + i]); }
+    HB_TRY(hb_scale_down(two.data(), (int)two.size(), K.Sp.data(), (int)K.Sp.size(), S, nS, ptxt_space));
+  }
+  return HB_OK;
+}
+
+// bringToSet(S) of each ciphertext's two parts and its self-tensor: HElib's squaring multLowLvl (src/Ctxt.cpp:1704-1708,
+// 1748-1751) before reLinearize, on checked arguments.  (a0, a1) over S_in become (a0^2, 2*a0*a1) over S and o2 receives
+// a1^2, all canonical.  norms (optional, [2*nitems]): norms[2i + k] = ||delta/P|| of part k of item i, from the same
+// conversion and norm_chunk as hb_scale_down_norm (0 when nothing is dropped).
+// Register path (power-of-two m, something dropped): per chunk, the inverse blk phase and the conversion of the 2*nit parts
+// into adjacent scratch slots (2i, 2i+1), then one k1_fwd_blk_square pass that finishes both rescales and writes the three
+// products -- as rescale_tensor_v1 does for two operands.  Otherwise scale_down_impl of the parts (lazy rows only where
+// k1_tensor follows) and hb_tensor(a0, a1, a0, a1 -> a0, a1, o2): k1_tensor and HB_PW_TENSOR read all four inputs of a
+// position before they write any output there, so the in-place self-tensor is exact.
+static int square_tensor_impl(hb_ctx* c, hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* o2, int nitems,
+                              const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space, double* norms) {
+  if (norms) std::fill(norms, norms + 2 * (size_t)nitems, 0.0);
+  if (v1_blk_ok(c) && !c->gen.on && nS < nS_in) {   // S is a strict subset of S_in: something is dropped
+    std::vector<int32_t> diff, kept; std::vector<u64> sc;
+    HB_TRY(scale_down_sets(c, S_in, nS_in, S, nS, ptxt_space, diff, kept, sc));
+    HB_TRY(ctx_scratch(c));
+    const int per = std::max(1, g_chunk / 2);   // items per chunk (the scratch holds HB_MAXB >= 2 parts)
+    for (int i0 = 0; i0 < nitems; i0 += per) {
+      const int nit = std::min(per, nitems - i0);
+      u64* P[HB_MAXB]; u64* tB[HB_MAXB]; u64* O2[HB_MAXB];
+      for (int i = 0; i < nit; i++) { P[2 * i] = a0[i0 + i]->d; P[2 * i + 1] = a1[i0 + i]->d; O2[i] = o2[i0 + i]->d; }
+      tmp_ptrs(c, c->tmpB, 2 * nit, tB);
+      HB_TRY(conv_chunk(c, P, 2 * nit, diff.data(), (int)diff.size(), kept.data(), (int)kept.size(), ptxt_space, 0, norms != nullptr));
+      HB_TRY(launch_blk_square_v1(c, (const u64* const*)tB, P, O2, nit, kept.data(), (int)kept.size(), sc.data()));
+      if (norms) HB_TRY(norm_chunk(c, 2 * nit, norms + 2 * (size_t)i0));
+    }
+    return HB_OK;
+  }
+  std::vector<hb_poly*> parts;
+  for (int i = 0; i < nitems; i++) { parts.push_back(a0[i]); parts.push_back(a1[i]); }
+  HB_TRY(scale_down_impl(parts.data(), (int)parts.size(), S_in, nS_in, S, nS, ptxt_space, norms, c->gen.on ? 0 : 1));
+  return hb_tensor(a0, a1, a0, a1, a0, a1, o2, nitems, S, nS);
+}
+// The checks shared by the squaring entry points: the operand polys and S within S_in.  The operands are rescaled in place,
+// so each poly may appear once only.
+static int square_check_args(hb_poly* const* a0, hb_poly* const* a1, int nitems, const int32_t* S_in, int nS_in, const int32_t* S, int nS,
+                             uint64_t ptxt_space, const char* who, hb_ctx** c, std::set<const hb_poly*>& in) {
+  if (nitems <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: nitems must be positive", who);
+  HB_TRY(check_polys(a0, nitems, c, who)); HB_TRY(check_polys(a1, nitems, c, who));
+  HB_TRY(check_idx(*c, S_in, nS_in, who)); HB_TRY(check_idx(*c, S, nS, who));
+  for (int i = 0; i < nS; i++)
+    if (std::find(S_in, S_in + nS_in, S[i]) == S_in + nS_in)
+      return hb_fail(HB_ERR_INDEX_SET, "%s: the target set must be a subset of the operands' set (prime %d)", who, S[i]);
+  if (ptxt_space < 1) return hb_fail(HB_ERR_BAD_ARG, "%s: ptxt_space must be at least 1", who);
+  in.clear(); in.insert(a0, a0 + nitems); in.insert(a1, a1 + nitems);
+  if (in.size() != 2 * (size_t)nitems) return hb_fail(HB_ERR_BAD_ARG, "%s: the operand polys must be distinct", who);
+  return HB_OK;
+}
+static int square_tensor_entry(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* o2, int nitems, const int32_t* S_in, int nS_in,
+                               const int32_t* S, int nS, uint64_t ptxt_space, double* norms, const char* who) {
+  hb_ctx* c = nullptr;
+  std::set<const hb_poly*> in;
+  HB_TRY(square_check_args(a0, a1, nitems, S_in, nS_in, S, nS, ptxt_space, who, &c, in));
+  HB_TRY(check_polys(o2, nitems, &c, who));
+  HB_TRY(check_outputs(in, {o2}, nitems, who));
+  // ---- every argument is checked: nothing was launched before this point
+  return square_tensor_impl(c, a0, a1, o2, nitems, S_in, nS_in, S, nS, ptxt_space, norms);
+}
+extern "C" int hb_square_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* o2, int nitems, const int32_t* S_in, int nS_in,
+                                const int32_t* S, int nS, uint64_t ptxt_space) {
+  return square_tensor_entry(a0, a1, o2, nitems, S_in, nS_in, S, nS, ptxt_space, nullptr, "hb_square_tensor");
+}
+extern "C" int hb_square_tensor_norm(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* o2, int nitems, const int32_t* S_in, int nS_in,
+                                     const int32_t* S, int nS, uint64_t ptxt_space, double* norms) {
+  if (!norms) return hb_fail(HB_ERR_BAD_ARG, "hb_square_tensor_norm: null output");
+  return square_tensor_entry(a0, a1, o2, nitems, S_in, nS_in, S, nS, ptxt_space, norms, "hb_square_tensor_norm");
+}
+
+// Ctxt::square (multiplyBy(*this), src/Ctxt.cpp:1757-1774 with the squaring branch of multLowLvl) of nitems ciphertexts
+// already at the target set's level, the squaring counterpart of hb_mul_relin_moddown: per chunk of items, the fused
+// rescale and self-tensor into (a0, a1) and one s^2 scratch poly per item (c->ip, shared with hb_inner_product), then
+// hb_relinearize's fused or step-by-step path over S | special, then the mod-down to S.
+extern "C" int hb_square_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, int nitems, const int32_t* S_in, int nS_in,
+                                       const int32_t* S, int nS, uint64_t ptxt_space, hb_poly* const* evk_a, hb_poly* const* evk_b,
+                                       int ndig_evk) {
+  static const char* who = "hb_square_relin_moddown";
+  hb_ctx* c = nullptr;
+  std::set<const hb_poly*> in;
+  HB_TRY(square_check_args(a0, a1, nitems, S_in, nS_in, S, nS, ptxt_space, who, &c, in));
+  if (c->special.empty()) return hb_fail(HB_ERR_BAD_ARG, "%s: context has no special primes", who);
+  KsSets K; HB_TRY(ks_sets(c, S, nS, who, K));
+  const KsKeys key = {1, nullptr, evk_a, evk_b, "evk"};
+  HB_TRY(ks_check_keys(c, &key, 1, K.nd, ndig_evk, K.Sp, who));
+  for (int i = 0; i < K.nd; i++)   // the operands are written while the key is read
+    if (in.count(evk_a[i]) || in.count(evk_b[i])) return hb_fail(HB_ERR_BAD_ARG, "%s: an operand aliases a key polynomial", who);
+  // ---- every argument is checked: nothing was launched before this point
+  std::vector<hb_poly*> ka; HB_TRY(ks_expand_a(c, evk_a, K.nd, K.Sp.data(), (int)K.Sp.size(), ka)); evk_a = ka.data();
+  const int G = std::min(nitems, c->chunk);
+  while ((int)c->ip.size() < G) { hb_poly* p; HB_TRY(hb_poly_create(c, &p)); c->ip.push_back(p); }
+  std::vector<hb_poly*> two;
+  for (int i0 = 0; i0 < nitems; i0 += G) {
+    const int nit = std::min(G, nitems - i0);
+    g_chunk = c->chunk;
+    HB_TRY(square_tensor_impl(c, a0 + i0, a1 + i0, c->ip.data(), nit, S_in, nS_in, S, nS, ptxt_space, nullptr));
+    // reLinearize (src/Ctxt.cpp:720-786)
+    HB_TRY(hb_relinearize(a0 + i0, a1 + i0, c->ip.data(), nit, S, nS, evk_a, evk_b, ndig_evk));
+    // drop the special primes again: modDownToSet(ctxtPrimes) (src/Ctxt.cpp:589-593)
+    two.clear();
+    for (int i = 0; i < nit; i++) { two.push_back(a0[i0 + i]); two.push_back(a1[i0 + i]); }
     HB_TRY(hb_scale_down(two.data(), (int)two.size(), K.Sp.data(), (int)K.Sp.size(), S, nS, ptxt_space));
   }
   return HB_OK;

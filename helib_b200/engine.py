@@ -368,6 +368,26 @@ class Engine:
                                            C.c_uint64(int(ptxt_space)), _arr(evk_a), _arr(evk_b), len(evk_a),
                                            _arr(out0), _arr(out1), int(bool(moddown))))
 
+    def square_tensor(self, a0, a1, o2, S_in, S, ptxt_space, norms=False):
+        """Per item i: (a0[i], a1[i]) over S_in brought to S and squared in place, a1[i]^2 into o2[i] (hb_square_tensor).
+        norms=True returns ||delta/P|| of each part, [item][part] (hb_square_tensor_norm)."""
+        x, pi, ni = _idx(S_in)
+        y, ps, ns = _idx(S)
+        if not norms:
+            self._ck(self.lib.hb_square_tensor(_arr(a0), _arr(a1), _arr(o2), len(a0), pi, ni, ps, ns, C.c_uint64(int(ptxt_space))))
+            return None
+        out = np.zeros(2 * len(a0), dtype=np.float64)
+        self._ck(self.lib.hb_square_tensor_norm(_arr(a0), _arr(a1), _arr(o2), len(a0), pi, ni, ps, ns, C.c_uint64(int(ptxt_space)),
+                                                out.ctypes.data_as(C.POINTER(C.c_double))))
+        return out.reshape(len(a0), 2)
+
+    def square_relin_moddown(self, a0, a1, S_in, S, ptxt_space, evk_a, evk_b):
+        """Per item i: (a0[i], a1[i]) over S_in squared, relinearised and modded down to S in place (hb_square_relin_moddown)."""
+        x, pi, ni = _idx(S_in)
+        y, ps, ns = _idx(S)
+        self._ck(self.lib.hb_square_relin_moddown(_arr(a0), _arr(a1), len(a0), pi, ni, ps, ns, C.c_uint64(int(ptxt_space)),
+                                                  _arr(evk_a), _arr(evk_b), len(evk_a)))
+
     def randomize(self, polys, idx, seed):
         """NTL::SetSeed(seed), then p.randomize() over rows idx for each p in polys, expanded on the device
         (hb_poly_randomize).  seed: the ZZ's little-endian magnitude bytes, or a non-negative int."""

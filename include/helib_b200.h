@@ -106,7 +106,7 @@ int hb_poly_randomize(hb_poly* const* polys, int npolys, const int32_t* idx, int
  * hb_poly_randomize (unsorted/duplicate idx, npolys <= 0, null seed with a length -> HB_ERR_BAD_ARG).
  * A seeded handle has no rows.  It is accepted in two places only: as an entry of evk_a of the key-switching entry points
  * (hb_keyswitch_digits, hb_keyswitch_digits_fused, hb_automorph_keyswitch_digits, hb_relinearize, hb_mul_relin_moddown,
- * hb_inner_product),
+ * hb_inner_product, hb_square_relin_moddown),
  * which regenerate the rows they read once per call into context scratch, and as `seeded` of hb_poly_expand.  Everything
  * else returns HB_ERR_BAD_ARG for it before launching anything; a key switch that needs a row outside the seeded set
  * returns HB_ERR_INDEX_SET.  hb_poly_destroy each handle; the shared schedule is freed with the last one and its bytes
@@ -401,7 +401,8 @@ int hb_relinearize(hb_poly* const* c0, hb_poly* const* c1, hb_poly* const* c2, i
 /* hb_mul_relin_moddown: operands (a0,a1),(b0,b1) over S_in; mod-down both to S (ptxt_space),
  * tensor, relinearise over S | special, mod-down the result to S.  Result in (a0,a1) rows S.
  * S is the common set of Ctxt::multiplyBy / multLowLvl (src/Ctxt.cpp:1700-1712) and must be a subset of S_in
- * (HB_ERR_INDEX_SET otherwise). */
+ * (HB_ERR_INDEX_SET otherwise).  The 4*nitems operand polys must be distinct (HB_ERR_BAD_ARG before any launch): the
+ * product is formed in place, so a ciphertext multiplied by itself needs a copy or hb_square_relin_moddown. */
 int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int nitems,
                          const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space,
                          hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk);
@@ -416,6 +417,26 @@ int hb_mul_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const*
 int hb_inner_product(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int npairs, int nitems,
                      const int32_t* S_in, int nS_in, const int32_t* S, int nS, uint64_t ptxt_space,
                      hb_poly* const* evk_a, hb_poly* const* evk_b, int ndig_evk, hb_poly* const* out0, hb_poly* const* out1, int moddown);
+/* hb_square_tensor: the squaring branch of Ctxt::multLowLvl (src/Ctxt.cpp:1704-1708, 1748-1751) for nitems ciphertexts
+ * (a0, a1) over S_in: both parts brought to S (bringToSet, S within S_in), then the self-tensor
+ *   a0 <- a0^2,   a1 <- 2*a0*a1,   o2 <- a1^2   (mod q, canonical, rows S).
+ * hb_square_tensor_norm also returns norms[2i + k] = ||delta/P||_canon of part k of item i, the double hb_scale_down_norm
+ * returns for that part (0 when S == S_in).  nitems <= 0, an operand poly given twice, o2 aliasing an operand or another
+ * output, a seeded handle, or a null norms -> HB_ERR_BAD_ARG; S not within S_in -> HB_ERR_INDEX_SET; all checked before
+ * any launch. */
+int hb_square_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* o2, int nitems, const int32_t* S_in, int nS_in,
+                     const int32_t* S, int nS, uint64_t ptxt_space);
+int hb_square_tensor_norm(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* o2, int nitems, const int32_t* S_in, int nS_in,
+                          const int32_t* S, int nS, uint64_t ptxt_space, double* norms);
+/* hb_square_relin_moddown: Ctxt::square (multiplyBy(*this)) of nitems ciphertexts, the fixed-set counterpart of
+ * hb_mul_relin_moddown: (a0, a1) over S_in are brought to S, squared, relinearised over S | special and modded down to S;
+ * the result is in (a0, a1) rows S, bit for bit what hb_mul_relin_moddown(x, copy of x) leaves.  No relin_CKKS_adjust (the
+ * Ctxt layer applies it).  Errors as hb_square_tensor, and: no special primes, too few matrix columns, an operand aliasing
+ * a key -> HB_ERR_BAD_ARG; S not within the ctxt primes, or a seeded evk_a without a needed row -> HB_ERR_INDEX_SET; all
+ * checked before any launch.  Stream-ordered; after the first call, a call of the same shape allocates nothing. */
+int hb_square_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, int nitems, const int32_t* S_in, int nS_in,
+                            const int32_t* S, int nS, uint64_t ptxt_space, hb_poly* const* evk_a, hb_poly* const* evk_b,
+                            int ndig_evk);
 
 #ifdef __cplusplus
 }
