@@ -226,6 +226,35 @@ template <int N> __device__ __forceinline__ void hb1_cp_wait() {
 #endif
 }
 
+// 128-byte shared->global bulk copy (TMA, bulk_group completion): the issuing thread does not wait for the global write,
+// so a warp that stores a scattered tile this way goes back to the network instead of stalling on its store queue.
+// Both addresses are multiples of 16 bytes.  The writes to the shared source must be fenced into the async proxy first.
+__device__ __forceinline__ void hb1_bulk_store128(u64* gdst, const u64* ssrc) {
+#ifdef HB_SIM
+  for (int i = 0; i < 16; i++) gdst[i] = ssrc[i];
+#else
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], 128;"
+               ::"l"(gdst), "r"((unsigned)__cvta_generic_to_shared(ssrc)) : "memory");
+  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void hb1_fence_async() {
+#ifndef HB_SIM
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+#endif
+}
+// the bulk copies of this thread have read their shared source (wait_read) / completed their global writes (wait_all)
+__device__ __forceinline__ void hb1_bulk_wait_read() {
+#ifndef HB_SIM
+  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void hb1_bulk_wait_all() {
+#ifndef HB_SIM
+  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+#endif
+}
+
 #define HB1_STAGE (16 * HB1_BS + 8)   // u64 per staging/exchange buffer
 
 // Work decomposition of the "blk" kernels: unit = (row, group of 16 blocks, batch item), numbered
@@ -249,7 +278,9 @@ __device__ __forceinline__ Hb1Unit hb1_unit(long u, int G, int nitems) {
 // Forward "blk" phase, 16 blocks per unit, persistent CTAs (grid.x CTAs, 256 threads).
 // Software pipelined: each thread prefetches its own 16 inputs of the NEXT unit (and, for the
 // mod-down epilogue, the 16 old destination values of the CURRENT unit) into shared memory with
-// cp.async while it computes; the staging tile doubles as the exchange tile.
+// cp.async while it computes; the staging tile doubles as the exchange tile.  The output rows go out as 128-byte bulk
+// copies from shared memory (the epilogue's row from O, the plain row from the exchange tile just read): 8-byte stores
+// scattered over 256 natural-order pieces held every warp at its store queue, so the network and the stores did not overlap.
 // smem: S[2][HB1_STAGE] | O[16][256] | TW1[256]
 template <bool SP>
 __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT Hb1BlkJob J) {
@@ -327,19 +358,33 @@ __global__ void __launch_bounds__(256, 2) k1_fwd_blk(const HbPrimeDev* __restric
     hb1_unroll<16>([&](auto l) { a[l] = Sb[blk2 * HB1_BS + HB1_RS * hi + l]; });
     hb1_r16_fwd<SP>(a, tw2, M);
     hb1_cp_wait<1>();   // old destination values (epilogue) have landed
+    // Output rows leave through 128-byte bulk stores from shared memory, value (l, hi) of the unit at T[l * 256 + tid], so
+    // T[l * 256 + 16 * h ..] is the natural-order piece brev8(16 * h + l) * N1 + [16 blocks]: the epilogue's row from O
+    // (each value over its own old value), the plain row from Sb once the exchange reads of every thread are done.
     hb1_unroll<16>([&](auto l) {
-      const size_t o = (size_t)((hb1_brev4(l) << 4) | hrev) << n1;   // brev8(16*hi + l) * N1
       if (epi) {
         u64 v = hb1_shoup4<SP>(O[l * 256 + tid] - a[l] + (M.qb2 + M.qb), sc, sc_s, M);   // (old - x) * P^-1, x in [0, 8q + 2^32), old < 4q
         if (!lazy) v = hb1_canon4(v, q);
-        old[o] = v;
+        O[l * 256 + tid] = v;
       }
-      if (!epi1) dst[o] = lazy ? a[l] : hb1_canon_fwd(a[l], q, M.qb);
+      if (!epi1 && !lazy) a[l] = hb1_canon_fwd(a[l], q, M.qb);
     });
     __syncthreads();   // exchange reads of Sb / TW1 done before they are overwritten
+    if (!epi1) hb1_unroll<16>([&](auto l) { Sb[l * 256 + tid] = a[l]; });
+    hb1_fence_async();
+    __syncthreads();
+    {   // thread (l, h) = (tid >> 4, tid & 15) sends piece (l, h) of each output row
+      const int l = tid >> 4, h = tid & 15;
+      const size_t o = (size_t)((hb1_brev4(l) << 4) | hb1_brev4(h)) << n1;
+      if (epi) hb1_bulk_store128(old - blk2 + o, O + l * 256 + 16 * h);
+      if (!epi1) hb1_bulk_store128(dst - blk2 + o, Sb + l * 256 + 16 * h);
+      hb1_bulk_wait_read();
+    }
+    __syncthreads();   // O and Sb are read out before the next unit's copies land in them
     cur = nxt;
   }
   hb1_cp_wait<0>();
+  hb1_bulk_wait_all();
 }
 
 // Rescale of a multiplication's four operand parts and their tensor product in one forward blk pass (scaleDownToSet of
