@@ -2010,7 +2010,10 @@ extern "C" int hb_conv_make_y_bcast(hb_poly* const* polys, int nitems, const int
   HB_TRY(check_idx(c, D, nD, "hb_conv_make_y_bcast")); HB_TRY(check_idx(c, owned, nOwned, "hb_conv_make_y_bcast(owned)", true));
   if (c->gen.on) return hb_fail(HB_ERR_UNSUPPORTED, "prime-sharded conversion is only built for power-of-two m");
   if (npeers < 0 || npeers > HB_MAXPEERS || (npeers && !peer_ypolys)) return hb_fail(HB_ERR_BAD_ARG, "hb_conv_make_y_bcast: npeers out of range");
-  for (int i = 0; i < npeers * nitems; i++) if (peer_ypolys[i]) HB_TRY(check_dense(peer_ypolys[i], "hb_conv_make_y_bcast(peers)"));
+  for (int i = 0; i < npeers * nitems; i++) {   // every peer slot is stored through: a null one is refused here, not dereferenced later
+    if (!peer_ypolys[i]) return hb_fail(HB_ERR_BAD_ARG, "hb_conv_make_y_bcast: null peer polynomial handle");
+    HB_TRY(check_dense(peer_ypolys[i], "hb_conv_make_y_bcast(peers)"));
+  }
   if (nOwned == 0) return HB_OK;
   if (nOwned > HB_MAXROWS) return hb_fail(HB_ERR_UNSUPPORTED, "hb_conv_make_y_bcast: more than %d owned rows", HB_MAXROWS);
   std::vector<u64> sc(nOwned);

@@ -150,6 +150,14 @@ class Engine:
             self.lib.hb_ctx_destroy(self.h)
             self.h = None
 
+    def __del__(self):
+        # every Poly holds its engine, so an engine is collected only after its polys: the context's device memory (the
+        # phase scratch alone is 2 x 64 x nprimes x N words) goes with it instead of staying allocated until the process exits
+        try:
+            self.close()
+        except Exception:
+            pass
+
     def _ck(self, rc):
         if rc != 0:
             raise HbError(rc, self.lib.hb_last_error().decode())
