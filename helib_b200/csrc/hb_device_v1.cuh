@@ -1019,3 +1019,74 @@ __global__ void __launch_bounds__(256) k1_tensor_sum(const HbPrimeDev* __restric
   hb1_st2(J.o2[it] + o, hb_reduce128(h2x, l2x, P), hb_reduce128(h2y, l2y, P));
 }
 
+// ------------------------------------------------------------------------------------------
+// Scaled sums of two-part ciphertexts (polyEval's simplePolyEval leaves, src/polyEval.cpp:223-255, as one linear pass):
+//   out_k[t][j] (+)= sum_i scal[j][i][r] * in_k[t][i]  (+ cst[j][r] on part 0)   (mod q_r, k = 0, 1)
+// on every row r of a set U.  The scalars and constants are canonical residues mod q_r, shared by the items; a zero scalar
+// means the input row is not read (an input over a smaller prime set contributes nothing there).  The job's tables live in
+// context-owned device memory: scal[(j*nin + i)*nU + r], cst[j*nU + r] (or null), the inputs of item t at in0/in1[t*nin + i]
+// and its outputs at out0/out1[t*nout + j].  One thread per coefficient: it reduces the words of every input that some
+// output reads on this row to [0, q) (any 64-bit word is accepted) and keeps them in shared memory (ni inputs x 2 parts x
+// blockDim words), then forms every output from them, so each input row is read once and each output row written once.
+// Each product is below 2^120, so the 128-bit sums carry on canonical every HB_TSUM_GROUP inputs; old outputs (accumulate)
+// may be any 64-bit values and the outputs are canonical.  Inputs [i0, i0 + ni) of the job take part in this launch.
+// grid = (ceil(N / blockDim), rows of the launch, items of the launch)
+#define HB_SSUM_SMEM (96 * 1024)                   // dynamic shared memory of k1_scaled_sums at most
+#define HB_SSUM_MAXIN (HB_SSUM_SMEM / (16 * 32 + 1))  // inputs one launch stages (32 threads): later groups accumulate
+struct Hb1ScaledSumsJob {
+  u64 N;
+  HbRows rows;        // prime indices of the launch's rows
+  int r0;             // position of rows.prime[0] in U
+  int nU, nin, nout, i0, ni, item0, accumulate, with_cst;
+  const u64* scal; const u64* cst;
+  const u64* const* in0; const u64* const* in1;
+  u64* const* out0; u64* const* out1;
+};
+__global__ void __launch_bounds__(256) k1_scaled_sums(const HbPrimeDev* __restrict__ primes, const HB_GRID_CONSTANT Hb1ScaledSumsJob J) {
+  HB_SMEM_DECL
+  u64* X = HB_SMEM;                                     // [ni][2][blockDim]
+  unsigned char* used = (unsigned char*)(X + (size_t)J.ni * 2 * blockDim.x);   // [ni]
+  const int pi = J.rows.prime[blockIdx.y];
+  const int r = J.r0 + blockIdx.y;
+  const HbPrimeDev P = primes[pi];
+  const int it = J.item0 + blockIdx.z;
+  const int T = blockDim.x, tid = threadIdx.x;
+  for (int i = tid; i < J.ni; i += T) {   // does any output read input i on this row?
+    unsigned char u = 0;
+    for (int j = 0; j < J.nout && !u; j++) u = __ldg(J.scal + ((size_t)j * J.nin + J.i0 + i) * J.nU + r) != 0;
+    used[i] = u;
+  }
+  __syncthreads();
+  const size_t c = (size_t)blockIdx.x * T + tid;
+  if (c >= J.N) return;
+  const size_t o = (size_t)pi * J.N + c;
+  for (int i = 0; i < J.ni; i++) {
+    u64 a = 0, b = 0;
+    if (used[i]) {
+      const size_t s = (size_t)it * J.nin + J.i0 + i;
+      a = hb1_canon(J.in0[s][o], P); b = hb1_canon(J.in1[s][o], P);
+    }
+    X[(size_t)(2 * i) * T + tid] = a; X[(size_t)(2 * i + 1) * T + tid] = b;
+  }
+  for (int j = 0; j < J.nout; j++) {
+    u64 h0 = 0, l0 = 0, h1 = 0, l1 = 0;
+    u64* const d0 = J.out0[(size_t)it * J.nout + j] + o;
+    u64* const d1 = J.out1[(size_t)it * J.nout + j] + o;
+    if (J.accumulate) { l0 = *d0; l1 = *d1; }
+    if (J.with_cst) { const u64 k = __ldg(J.cst + (size_t)j * J.nU + r); l0 += k; h0 += l0 < k; }
+    const u64* sc = J.scal + ((size_t)j * J.nin + J.i0) * J.nU + r;
+    for (int g0 = 0; g0 < J.ni; g0 += HB_TSUM_GROUP) {
+      if (g0 > 0) { l0 = hb_reduce128(h0, l0, P); l1 = hb_reduce128(h1, l1, P); h0 = h1 = 0; }   // carry on canonical
+      const int g1 = J.ni - g0 < HB_TSUM_GROUP ? J.ni : g0 + HB_TSUM_GROUP;
+      for (int i = g0; i < g1; i++) {
+        const u64 s = __ldg(sc + (size_t)i * J.nU);
+        if (s == 0) continue;
+        hb1_mac128(h0, l0, s, X[(size_t)(2 * i) * T + tid]);
+        hb1_mac128(h1, l1, s, X[(size_t)(2 * i + 1) * T + tid]);
+      }
+    }
+    *d0 = hb_reduce128(h0, l0, P);
+    *d1 = hb_reduce128(h1, l1, P);
+  }
+}
+

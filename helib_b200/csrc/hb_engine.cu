@@ -129,6 +129,7 @@ struct hb_ctx {
   std::vector<hb_poly*> block;  // hb_block_linear_map: rotations, rotated sums, digits and set-1 sums (first use)
   std::vector<hb_poly*> ip;     // hb_inner_product: the s^2 part of each item of a chunk (first use)
   std::vector<hb_poly*> leaf;   // hb_full_linear_map_leaves: cleaned leaves, their digits, per-leaf sums, final matrix (first use)
+  u64* ssum = nullptr; size_t ssum_cap = 0;   // hb_ctxt_scaled_sums: its scalar, constant and pointer tables (grown on demand)
 };
 // The row schedule of a seeded set (hb_poly_create_seeded): the ChaCha20 key, the rows, and in one device allocation the
 // first buffer of every schedule row (start[T+1]) and the exclusive row offset of every counted buffer (off[T*wmax]).
@@ -333,6 +334,7 @@ static int ctx_build(hb_ctx* c, hb_ctx** out, int device, uint64_t m, int nprime
   HB_CUDA(cudaFuncSetAttribute(k1_conv1<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
   HB_CUDA(cudaFuncSetAttribute(k1_conv1<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024));
   HB_CUDA(cudaFuncSetAttribute(k1_conv<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+  HB_CUDA(cudaFuncSetAttribute(k1_scaled_sums, cudaFuncAttributeMaxDynamicSharedMemorySize, HB_SSUM_SMEM));
   HB_CUDA(cudaFuncSetAttribute(k1_conv<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
   HB_CUDA(cudaFuncSetAttribute(k1_fwd_blk<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 112 * 1024));
@@ -363,6 +365,7 @@ extern "C" void hb_ctx_destroy(hb_ctx* c) {
   for (hb_poly* p : c->bsgs) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->block) { cudaFree(p->d); delete p; }
   for (hb_poly* p : c->leaf) { cudaFree(p->d); delete p; }
+  cudaFree(c->ssum);
   for (hb_poly* p : c->ip) { cudaFree(p->d); delete p; }
   for (HbTmap* sl : c->tmap_slabs) cudaFree(sl);
   if (c->own_stream) cudaStreamDestroy(c->own_stream);
@@ -3471,4 +3474,85 @@ extern "C" int hb_square_relin_moddown(hb_poly* const* a0, hb_poly* const* a1, i
     HB_TRY(square_tensor_impl(c, a0 + i0, a1 + i0, c->ip.data(), nit, S_in, nS_in, S, nS, ptxt_space, nullptr));
     return relin_moddown(a0 + i0, a1 + i0, c->ip.data(), nit, S, nS, K, ptxt_space, evk_a, evk_b, ndig_evk, true);
   });
+}
+
+// ------------------------------------------------------------------------------------------
+// hb_ctxt_scaled_sums: k1_scaled_sums on checked arguments.  The tables travel to the context's device buffer in one
+// stream-ordered copy (pageable: cudaMemcpyAsync has staged them when it returns, so the caller may free its arrays); the
+// buffer only grows.  A launch covers at most HB_MAXROWS rows and HB_MAXB item-output pairs (one item at least, with all
+// its outputs, so that every input row is read once); more than HB_SSUM_MAXIN inputs (the shared-memory stage of one
+// thread group) run as input groups, the later ones accumulating into the outputs.
+static int scaled_sums_impl(hb_ctx* c, hb_poly* const* in0, hb_poly* const* in1, int nin, hb_poly* const* out0, hb_poly* const* out1,
+                            int nout, int nitems, const int32_t* U, int nU, const uint64_t* scal, const uint64_t* cst, int accumulate) {
+  const size_t nsc = (size_t)nout * nin * nU, ncst = cst ? (size_t)nout * nU : 0;
+  const size_t npi = (size_t)nitems * nin, npo = (size_t)nitems * nout;
+  const size_t words = nsc + ncst + 2 * npi + 2 * npo;
+  if (words > c->ssum_cap) {
+    if (c->ssum) { HB_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(c->ssum); c->bytes -= c->ssum_cap * 8; c->ssum = nullptr; c->ssum_cap = 0; }
+    HB_TRY(ctx_alloc(c, (void**)&c->ssum, words * 8));
+    c->ssum_cap = words;
+  }
+  std::vector<u64> h(words);
+  memcpy(h.data(), scal, nsc * 8);
+  if (cst) memcpy(h.data() + nsc, cst, ncst * 8);
+  u64* pt = h.data() + nsc + ncst;
+  for (size_t e = 0; e < npi; e++) { pt[e] = (u64)(uintptr_t)in0[e]->d; pt[npi + e] = (u64)(uintptr_t)in1[e]->d; }
+  for (size_t e = 0; e < npo; e++) { pt[2 * npi + e] = (u64)(uintptr_t)out0[e]->d; pt[2 * npi + npo + e] = (u64)(uintptr_t)out1[e]->d; }
+  HB_CUDA(cudaMemcpyAsync(c->ssum, h.data(), words * 8, cudaMemcpyHostToDevice, c->stream));
+  const u64* d = c->ssum;
+  const int per = std::max(1, HB_MAXB / nout);   // items per launch
+  for (int g0 = 0; g0 < nin; g0 += HB_SSUM_MAXIN) {
+    const int ni = std::min(HB_SSUM_MAXIN, nin - g0);
+    int T = 256;   // threads per block: the largest whose stage fits HB_SSUM_SMEM / 3 (HB_SSUM_SMEM for 32 threads)
+    while (T > 32 && (size_t)ni * (16 * T + 1) > HB_SSUM_SMEM / 3) T >>= 1;
+    const size_t smem = (size_t)ni * (16 * T + 1);
+    for (int t0 = 0; t0 < nitems; t0 += per) {
+      const int nt = std::min(per, nitems - t0);
+      for (int r0 = 0; r0 < nU; r0 += HB_MAXROWS) {
+        const int nr = std::min(HB_MAXROWS, nU - r0);
+        Hb1ScaledSumsJob J; memset(&J, 0, sizeof(J));
+        J.N = c->N; fill_rows(J.rows, U + r0, nr); J.r0 = r0;
+        J.nU = nU; J.nin = nin; J.nout = nout; J.i0 = g0; J.ni = ni; J.item0 = t0;
+        J.accumulate = accumulate || g0 > 0; J.with_cst = cst != nullptr && g0 == 0;
+        J.scal = d; J.cst = cst ? d + nsc : nullptr;
+        J.in0 = (const u64* const*)(d + nsc + ncst); J.in1 = J.in0 + npi;
+        J.out0 = (u64* const*)(d + nsc + ncst + 2 * npi); J.out1 = J.out0 + npo;
+        u64 rd = 0;   // algorithmic bytes: the input rows some output reads, the outputs written (and read back)
+        for (int k = 0; k < nr; k++)
+          for (int i = g0; i < g0 + ni; i++)
+            for (int j = 0; j < nout; j++) if (scal[((size_t)j * nin + i) * nU + r0 + k]) { rd += 2; break; }
+        const u64 bytes = (rd + (u64)2 * nout * nr * (J.accumulate ? 2 : 1)) * nt * c->N * 8;
+        pre_launch(c);
+        HB_LAUNCH(k1_scaled_sums, dim3((unsigned)((c->N + T - 1) / T), nr, nt), dim3(T), smem, c->stream, c->d_primes, J);
+        HB_TRY(post_launch(c, "k1_scaled_sums", bytes));
+      }
+    }
+  }
+  return HB_OK;
+}
+extern "C" int hb_ctxt_scaled_sums(hb_poly* const* in0, hb_poly* const* in1, int nin, hb_poly* const* out0, hb_poly* const* out1,
+                                   int nout, int nitems, const int32_t* U, int nU, const uint64_t* scal, const uint64_t* cst,
+                                   int accumulate) {
+  static const char* who = "hb_ctxt_scaled_sums";
+  if (nin <= 0 || nout <= 0 || nitems <= 0 || nU <= 0) return hb_fail(HB_ERR_BAD_ARG, "%s: nin, nout, nitems and nU must be positive", who);
+  if (accumulate != 0 && accumulate != 1) return hb_fail(HB_ERR_BAD_ARG, "%s: accumulate must be 0 or 1", who);
+  if (!U || !scal) return hb_fail(HB_ERR_BAD_ARG, "%s: null row set or scalar table", who);
+  hb_ctx* c = nullptr;
+  const int np = nin * nitems, no = nout * nitems;
+  HB_TRY(check_polys(in0, np, &c, who)); HB_TRY(check_polys(in1, np, &c, who));
+  HB_TRY(check_polys(out0, no, &c, who)); HB_TRY(check_polys(out1, no, &c, who));
+  for (int r = 0; r < nU; r++) {
+    if (U[r] < 0 || U[r] >= c->nprimes) return hb_fail(HB_ERR_INDEX_SET, "%s: prime index %d outside the chain", who, U[r]);
+    if (r > 0 && U[r] <= U[r - 1]) return hb_fail(HB_ERR_INDEX_SET, "%s: the row set must be sorted without repeats", who);
+  }
+  for (int j = 0; j < nout; j++)
+    for (int r = 0; r < nU; r++) {
+      const u64 q = c->q[U[r]];
+      if (cst && cst[(size_t)j * nU + r] >= q) return hb_fail(HB_ERR_BAD_ARG, "%s: constant %d of row %d is not below its prime", who, j, r);
+      for (int i = 0; i < nin; i++)
+        if (scal[((size_t)j * nin + i) * nU + r] >= q) return hb_fail(HB_ERR_BAD_ARG, "%s: scalar (%d, %d) of row %d is not below its prime", who, j, i, r);
+    }
+  std::set<const hb_poly*> in(in0, in0 + np); in.insert(in1, in1 + np);
+  HB_TRY(check_outputs(in, {out0, out1}, no, who));
+  return scaled_sums_impl(c, in0, in1, nin, out0, out1, nout, nitems, U, nU, scal, cst, accumulate);
 }

@@ -364,6 +364,21 @@ class Engine:
         self._ck(self.lib.hb_tensor_sum(_arr(fl[0]), _arr(fl[1]), _arr(fl[2]), _arr(fl[3]), npairs, len(a0), p, n,
                                         _arr(o0), _arr(o1), _arr(o2), int(bool(accumulate))))
 
+    def ctxt_scaled_sums(self, in0, in1, out0, out1, U, scal, cst=None, accumulate=False):
+        """Per item t and output j, on every row r of U: (out0, out1)[t][j] (+)= sum_i scal[j, i, r] * (in0, in1)[t][i],
+        plus cst[j, r] on part 0 (hb_ctxt_scaled_sums).  in0/in1: one list of nin inputs per item; out0/out1: one list of
+        nout outputs per item; scal: (nout, nin, len(U)) canonical residues; cst: (nout, len(U)) or None."""
+        nin = len(in0[0]) if in0 else 0
+        nout = len(out0[0]) if out0 else 0
+        fi = [[p for item in x for p in item] for x in (in0, in1)]
+        fo = [[p for item in x for p in item] for x in (out0, out1)]
+        a, p, n = _idx(U)
+        sc = np.ascontiguousarray(np.asarray(scal, dtype=np.uint64))
+        cs = None if cst is None else np.ascontiguousarray(np.asarray(cst, dtype=np.uint64))
+        self._ck(self.lib.hb_ctxt_scaled_sums(_arr(fi[0]), _arr(fi[1]), nin, _arr(fo[0]), _arr(fo[1]), nout, len(in0), p, n,
+                                              sc.ctypes.data_as(u64p), cs.ctypes.data_as(u64p) if cs is not None else None,
+                                              int(bool(accumulate))))
+
     def inner_product(self, a0, a1, b0, b1, S_in, S, ptxt_space, evk_a, evk_b, out0, out1, moddown=True):
         """Per item t: sum_j (a0,a1)[t][j] * (b0,b1)[t][j] brought to S, relinearised once into (out0[t], out1[t]) over
         S | special, and with moddown over S (hb_inner_product).  Operands over S_in are brought to S in place."""

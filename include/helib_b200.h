@@ -347,6 +347,22 @@ int hb_tensor(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_pol
  * npairs or nitems <= 0, accumulate not 0/1, or an output aliasing an input or another output -> HB_ERR_BAD_ARG. */
 int hb_tensor_sum(hb_poly* const* a0, hb_poly* const* a1, hb_poly* const* b0, hb_poly* const* b1, int npairs, int nitems,
                   const int32_t* idx, int n, hb_poly* const* o0, hb_poly* const* o1, hb_poly* const* o2, int accumulate);
+/* Scaled sums of two-part ciphertexts: every simplePolyEval leaf of polyEval (src/polyEval.cpp:223-255) is
+ * sum_i s_i * X^i + c on every row, with per-row integer scalars that the loop's multByConstant / modUpToSet / addCtxt /
+ * addConstant arithmetic determines.  nitems items, each with nin inputs (in0, in1)[t*nin + i] and nout outputs
+ * (out0, out1)[t*nout + j]; on every row r of U (sorted, no repeats, within the chain):
+ *   out_k[t*nout + j] (+)= sum_i scal[(j*nin + i)*nU + r] * in_k[t*nin + i]   (mod q_{U[r]}, k = 0, 1)
+ * plus cst[j*nU + r] on part 0 (cst may be NULL).  accumulate = 0 overwrites.  The items share scal and cst, which are
+ * canonical residues; a zero scalar means that input row is not read.  Inputs may be any 64-bit words (reduced on load);
+ * outputs are canonical.  Each input row is read once and each output row written once, for any nout (more than
+ * HB_SSUM_MAXIN = 191 inputs run in groups, the later ones accumulating).  The tables are staged in context-owned device
+ * memory in stream order: the call is asynchronous, the caller may free its arrays when it returns, and after the first
+ * call a call of the same shape allocates nothing.  Counts <= 0, accumulate not 0/1, a scalar or constant not below its
+ * prime, an output aliasing an input or another output, or a seeded handle -> HB_ERR_BAD_ARG; U unsorted, repeated or
+ * outside the chain -> HB_ERR_INDEX_SET; all checked before any launch. */
+int hb_ctxt_scaled_sums(hb_poly* const* in0, hb_poly* const* in1, int nin, hb_poly* const* out0, hb_poly* const* out1,
+                        int nout, int nitems, const int32_t* U, int nU, const uint64_t* scal, const uint64_t* cst,
+                        int accumulate);
 /* DoubleCRT::automorph (src/DoubleCRT.cpp:1160-1202): dst[j] = src[idx(rep(j)*k mod m)], dst != src */
 int hb_automorph(hb_poly* const* dst, hb_poly* const* src, int nitems, const int32_t* idx, int n, uint64_t k);
 
