@@ -17,6 +17,9 @@
 //   multLowLvl / multiplyBy        src/Ctxt.cpp:1681-1774
 //   modSwitchAddedNoiseBound       src/Ctxt.cpp:2560-2582
 //   polyEval / DynamicCtxtPowers   src/polyEval.cpp:18-29, 129-389   (every simplePolyEval leaf in one hb_ctxt_scaled_sums call)
+//   divideByP / multByP            src/Ctxt.cpp:2415-2435, include/helib/Ctxt.h:1216-1221
+//   extractDigits / extendExtract  src/extractDigits.cpp:28-308       (each round's subtract-and-divide chain in one call)
+//   extractDigitsThin              src/recryption.cpp:793-909        (its final combination in one call)
 #pragma once
 #include <algorithm>
 #include <cfloat>
@@ -690,6 +693,43 @@ class Ctxt {
     unsigned long q = 1;
     for (long i : primeSet) q = (unsigned long)(((unsigned __int128)q * (unsigned long)(context.ithPrime(i) % ptxtSpace)) % (unsigned long)ptxtSpace);
     return balRem((long)(((unsigned __int128)(unsigned long)intFactor * q) % (unsigned long)ptxtSpace), ptxtSpace);
+  }
+  // effectiveR (src/Ctxt.cpp:103-114): r with ptxtSpace = p^r
+  long effectiveR() const {
+    const long p = context.getP();
+    for (long r = 1, p2r = p; r < 60; r++, p2r *= p) {   // HELIB_SP_NBITS
+      if (p2r == ptxtSpace) return r;
+      if (p2r > ptxtSpace) break;
+    }
+    throw RuntimeError("ctxt.ptxtSpace is not of the form p^r");
+  }
+  // divideByP (src/Ctxt.cpp:2415-2435): every part times p^-1 mod Q, in one hb_scale_rows call over the parts; the
+  // plaintext space drops from p^r to p^(r-1).  The ciphertext must encrypt a multiple of p.
+  void divideByP() {
+    if (isEmpty()) return;
+    divideByPMeta();
+    const std::vector<int32_t> idx = primeSet.vec();
+    std::vector<uint64_t> sc;
+    for (int32_t i : idx) sc.push_back((uint64_t)invMod(context.getP(), context.ithPrime(i)));
+    std::vector<hb_poly*> d;   // every part is over primeSet (addPart and matchPrimeSet keep it so)
+    for (auto& part : parts) d.push_back(part.dcrt.handle());
+    if (!idx.empty()) check(hb_scale_rows(d.data(), (int)d.size(), idx.data(), (int)idx.size(), sc.data()));
+  }
+  // divideByP's asserts and metadata, the part the fused digit chains replay
+  void divideByPMeta() {
+    const long p = context.getP();
+    if (ptxtSpace % p != 0) throw LogicError("p must divide ptxtSpace");
+    if (!(ptxtSpace > p)) throw LogicError("ptxtSpace must be strictly greater than p");
+    noiseBound = noiseBound / XD((double)p);
+    ptxtSpace /= p;
+    intFactor %= ptxtSpace;
+  }
+  // multByP (include/helib/Ctxt.h:1216-1221): times p^e, the plaintext space grows to p^(r+e)
+  void multByP(long e = 1) {
+    long p2e = 1;
+    for (long i = 0; i < e; i++) p2e *= context.getP();
+    ptxtSpace *= p2e;
+    multByConstant(p2e);
   }
   long getKeyID() const { for (auto& part : parts) if (!part.skHandle.isOne()) return part.skHandle.secretKeyID; return 0; }   // src/Ctxt.cpp:2550-2557
   void cleanUp() {   // src/Ctxt.cpp:788-797
@@ -2438,6 +2478,453 @@ inline void polyEval(Ctxt& ret, std::vector<long> poly, const Ctxt& x, long k = 
     topTerm.multByConstant(extra);
     ret -= topTerm;
   }
+}
+
+// ---- digit extraction (src/extractDigits.cpp, src/recryption.cpp:793-909) ----------------------------------------------
+// The polynomials are computed on the host from their definitions: arithmetic mod p^e (p^e < 2^30) and, for Chen and Han's
+// a(m), mod p^(2e) < 2^60, in 128-bit products.
+namespace xd {
+using Poly = std::vector<long>;
+inline long mulmod(long a, long b, long q) { return (long)((unsigned __int128)(uint64_t)a * (uint64_t)b % (uint64_t)q); }
+inline long power(long p, long e) { long r = 1; for (long i = 0; i < e; i++) r *= p; return r; }
+inline long powmod(long a, long e, long q) { long r = 1 % q; for (a %= q; e; e >>= 1, a = mulmod(a, a, q)) if (e & 1) r = mulmod(r, a, q); return r; }
+inline Poly mulTrunc(const Poly& a, const Poly& b, long len, long q) {   // a*b mod (X^len, q)
+  Poly r((size_t)len, 0);
+  for (size_t i = 0; i < a.size() && (long)i < len; i++)
+    if (a[i]) for (size_t j = 0; j < b.size() && (long)(i + j) < len; j++) r[i + j] = (r[i + j] + mulmod(a[i], b[j], q)) % q;
+  return r;
+}
+// The unique f of degree < #x with f(x_j) = y_j mod p^e, coefficients in [0, p^e), for x_j distinct mod p
+// (interpolateMod, src/NumbTh.cpp:1043): its p-adic digits are interpolated one at a time mod p, lowest first.
+inline Poly interpolateMod(const std::vector<long>& x, std::vector<long> y, long p, long e) {
+  const size_t n = x.size();
+  const long p2e = power(p, e);
+  Poly res(n, 0);
+  for (auto& v : y) { v %= p2e; if (v < 0) v += p2e; }
+  std::vector<long> xm(n);
+  for (size_t j = 0; j < n; j++) { xm[j] = x[j] % p; if (xm[j] < 0) xm[j] += p; }
+  Poly M{1};   // prod_k (X - x_k) mod p
+  for (size_t k = 0; k < n; k++) {
+    Poly nb(M.size() + 1, 0);
+    for (size_t t = 0; t < M.size(); t++) { nb[t + 1] = (nb[t + 1] + M[t]) % p; nb[t] = (nb[t] + mulmod(M[t], (p - xm[k]) % p, p)) % p; }
+    M = nb;
+  }
+  std::vector<Poly> basis(n, Poly(n, 0));   // M / (X - x_j), scaled to 1 at x_j
+  for (size_t j = 0; j < n; j++) {
+    Poly& b = basis[j];
+    for (size_t t = n; t-- > 0;) b[t] = t + 1 == n ? M[n] : (M[t + 1] + mulmod(xm[j], b[t + 1], p)) % p;
+    long den = 0;
+    for (size_t t = n; t-- > 0;) den = (mulmod(den, xm[j], p) + b[t]) % p;
+    const long s = Ctxt::invMod(den, p);
+    for (auto& c : b) c = mulmod(c, s, p);
+  }
+  for (long pl = 1, mod = p2e; mod > 1; pl *= p, mod /= p) {
+    Poly g(n, 0);   // the lowest p-adic digits of y, interpolated mod p
+    for (size_t j = 0; j < n; j++) for (size_t t = 0; t < n; t++) g[t] = (g[t] + mulmod(basis[j][t], y[j] % p, p)) % p;
+    for (size_t t = 0; t < n; t++) res[t] += g[t] * pl;
+    for (size_t j = 0; j < n; j++) {   // y_j = (y_j - g(x_j) mod p^(e-lvl)) / p
+      long v = 0, xj = x[j] % mod; if (xj < 0) xj += mod;
+      for (size_t t = n; t-- > 0;) v = (mulmod(v, xj, mod) + g[t]) % mod;
+      long d = y[j] - v; if (d < 0) d += mod;
+      y[j] = d / p;
+    }
+  }
+  pe::normalize(res);
+  return res;
+}
+// buildDigitPolynomial (src/extractDigits.cpp:28-58): f = X^p + f' with f'(z) = z - z^p mod p^e for |z| <= p/2, so that
+// f(z0 + p^t z1) = z0 mod p^(t+1) for t < e.  Empty for p < 2 or e <= 1.
+inline Poly buildDigitPolynomial(long p, long e) {
+  if (p < 2 || e <= 1) return {};
+  const long p2e = power(p, e);
+  std::vector<long> x((size_t)p), y((size_t)p);
+  for (long j = 0; j < p; j++) {
+    const long z = -(p / 2) + j;
+    x[(size_t)j] = z;
+    long v = z - powmod(z < 0 ? z + p2e : z, p, p2e);
+    while (v > p2e / 2) v -= p2e;
+    while (v < -(p2e / 2)) v += p2e;
+    y[(size_t)j] = v;
+  }
+  Poly f = interpolateMod(x, y, p, e);
+  if (pe::deg(f) >= p) throw LogicError("Interpolation error.  Degree too high.");
+  pe::setCoeff(f, p);
+  return f;
+}
+// compute_a_vals (src/extractDigits.cpp:131-172): a[m] = a(m)/m! mod p^e for m = p .. (e-1)(p-1)+1, where the a(m) are the
+// coefficients of p (X+1)^p / ((X+1)^p - X^p) as a power series mod p^(2e)
+inline std::vector<long> chenHanA(long p, long e) {
+  const long pe_ = power(p, e), p2e = pe_ * pe_;
+  const long len = (e - 1) * (p - 1) + 2;
+  Poly xp1{1}, b{1, 1};   // (X+1)^p mod (X^len, p^(2e))
+  for (long k = p; k; k >>= 1) { if (k & 1) xp1 = mulTrunc(xp1, b, len, p2e); b = mulTrunc(b, b, len, p2e); }
+  Poly den = xp1;
+  if (p < len) den[(size_t)p] = (den[(size_t)p] - 1 + p2e) % p2e;
+  Poly inv((size_t)len, 0);   // 1/den mod X^len: den(0) = 1
+  for (long i = 0; i < len; i++) {
+    long s = i == 0 ? 1 : 0;
+    for (long j = 1; j <= i; j++) s = (s - mulmod(den[(size_t)j], inv[(size_t)(i - j)], p2e) + p2e) % p2e;
+    inv[(size_t)i] = s;
+  }
+  Poly poly = mulTrunc(xp1, inv, len, p2e);
+  for (auto& c : poly) c = mulmod(c, p, p2e);
+  std::vector<long> a((size_t)len, 0);
+  long mfac = 1;
+  for (long m = 2; m < p; m++) mfac = mulmod(mfac, m, p2e);
+  for (long m = p; m < len; m++) {
+    mfac = mulmod(mfac, m, p2e);
+    const long c = poly[(size_t)m];
+    long d = 1;   // gcd(mfac, p^(2e)), p^(2e) for mfac = 0
+    for (long t = mfac; d < p2e && t % p == 0; t /= p) { d *= p; if (t == 0) { d = p2e; break; } }
+    if (d > pe_ || c % d != 0) throw RuntimeError("cannot divide");
+    a[(size_t)m] = mulmod((c / d) % pe_, Ctxt::invMod((mfac / d) % pe_, pe_), pe_);
+  }
+  return a;
+}
+// compute_magic_poly (src/extractDigits.cpp:178-222): Chen and Han's G with G(x) = (x mod p) mod p^e, x mod p in [0, 1]
+// for p = 2 and in (-p/2, p/2) otherwise; coefficients in [0, p^e)
+inline Poly chenHanMagicPoly(long p, long e) {
+  const std::vector<long> a = chenHanA(p, e);
+  const long q = power(p, e), len = (e - 1) * (p - 1) + 2;
+  auto mulLin = [&](Poly& t, long m) {   // t *= (X - m)
+    Poly r(t.size() + 1, 0);
+    const long mm = (q - m % q) % q;
+    for (size_t i = 0; i < t.size(); i++) { r[i + 1] = (r[i + 1] + t[i]) % q; r[i] = (r[i] + mulmod(t[i], mm, q)) % q; }
+    t = r;
+  };
+  Poly term{1 % q}, poly;
+  for (long m = 0; m < p; m++) mulLin(term, m);
+  for (long m = p; m < len; m++) {
+    if (poly.size() < term.size()) poly.resize(term.size(), 0);
+    for (size_t i = 0; i < term.size(); i++) poly[i] = (poly[i] + mulmod(term[i], a[(size_t)m], q)) % q;
+    mulLin(term, m);
+  }
+  if (p % 2 == 1) {   // poly(X + (p-1)/2), by Horner
+    Poly p2;
+    for (long i = (long)poly.size() - 1; i >= 0; i--) {
+      mulLin(p2, -((p - 1) / 2));
+      if (p2.empty()) p2.push_back(0);
+      p2[0] = (p2[0] + poly[(size_t)i]) % q;
+    }
+    poly = p2;
+  }
+  for (auto& c : poly) c = (q - c) % q;   // X - poly
+  if (poly.size() < 2) poly.resize(2, 0);
+  poly[1] = (poly[1] + 1) % q;
+  pe::normalize(poly);
+  return poly;
+}
+}  // namespace xd
+
+// One linear combination of 2-part ciphertexts, formed in one hb_ctxt_scaled_sums call.  The operations of the digit
+// chains (addCtxt, divideByP, multByP, negate, reducePtxtSpace) are linear and exact on every row: the mod-up of addCtxt
+// multiplies the old rows by the added primes and leaves zero on the new ones, the intFactor harmonisation and multByP
+// multiply by small signed integers, divideByP by p^-1 mod q_r.  A Term replays them on the metadata (primeSet, ptxtSpace,
+// intFactor, noiseBound, ratFactor, ptxtMag) as the mirror's methods compute it, and keeps each input's scalar on every row.
+// `ok` turns false where the loop would throw; the caller then runs the loop, which throws as HElib does.
+class LinearChain {
+ public:
+  using u64 = uint64_t;
+  struct Term { Ctxt meta; std::vector<std::vector<u64>> s; };   // s[input][row]
+  bool ok = true;
+
+  // ok is false unless the inputs are BGV, non-empty, 2-part canonical under one key, with their parts over their primeSet
+  explicit LinearChain(std::vector<const Ctxt*> inputs) : in_(std::move(inputs)), ctx_(in_.at(0)->context), np_(ctx_.numPrimes()) {
+    const Ctxt& c0 = *in_[0];
+    keyID_ = c0.getKeyID();
+    for (const Ctxt* c : in_) {
+      if (c->isCKKS() || &c->pubKey != &c0.pubKey || c->parts.size() != 2 || !c->inCanonicalForm(keyID_) || c->getKeyID() != keyID_) ok = false;
+      else for (const auto& part : c->parts) if (!(part.dcrt.getIndexSet() == c->primeSet)) ok = false;
+    }
+  }
+  Term term(size_t k) const {
+    const Ctxt& c = *in_.at(k);
+    Term t{metaOf(c), std::vector<std::vector<u64>>(in_.size(), std::vector<u64>(np_, 0))};
+    for (long r : c.primeSet) t.s[k][(size_t)r] = 1;
+    return t;
+  }
+  // a += b or a -= b: Ctxt::addCtxt (src/Ctxt.cpp:1406-1556), BGV
+  void add(Term& a, Term b, bool negative = false) {
+    if (!ok) return;
+    const long g = std::gcd(a.meta.ptxtSpace, b.meta.ptxtSpace);
+    if (g <= 1) { ok = false; return; }
+    a.meta.reducePtxtSpace(b.meta.ptxtSpace);
+    if (b.meta.ptxtSpace != a.meta.ptxtSpace) b.meta.reducePtxtSpace(a.meta.ptxtSpace);
+    if (!modUp(a, b.meta.primeSet / a.meta.primeSet) || !modUp(b, a.meta.primeSet / b.meta.primeSet)) return;
+    long e1 = 1, e2 = 1;
+    if (a.meta.intFactor != b.meta.intFactor) Ctxt::harmoniseIntFactors(a.meta, b.meta, e1, e2);
+    mulInt(b, e2);
+    mulInt(a, e1);
+    for (size_t k = 0; k < in_.size(); k++)
+      for (long r : a.meta.primeSet) {
+        const u64 q = (u64)ctx_.ithPrime(r), x = b.s[k][(size_t)r];
+        a.s[k][(size_t)r] = negative ? (a.s[k][(size_t)r] + q - x) % q : (a.s[k][(size_t)r] + x) % q;
+      }
+    a.meta.ptxtMag = a.meta.ptxtMag + b.meta.ptxtMag;
+    a.meta.noiseBound = a.meta.noiseBound + b.meta.noiseBound;
+  }
+  void divideByP(Term& a) {   // Ctxt::divideByP
+    if (!ok) return;
+    const long p = ctx_.getP();
+    if (a.meta.ptxtSpace % p != 0 || !(a.meta.ptxtSpace > p)) { ok = false; return; }
+    a.meta.divideByPMeta();
+    for (long r : a.meta.primeSet) scaleRow(a, r, (u64)Ctxt::invMod(p, ctx_.ithPrime(r)));
+  }
+  void multByP(Term& a, long e = 1) {   // Ctxt::multByP, through multByConstant(long)'s BGV branch
+    if (!ok) return;
+    const long p2e = xd::power(ctx_.getP(), e);
+    Ctxt& m = a.meta;
+    m.ptxtSpace *= p2e;
+    const long c0 = p2e % m.ptxtSpace;
+    if (c0 == 1) return;
+    if (c0 == 0) { ok = false; return; }   // multByConstant clears the ciphertext
+    const long d = std::gcd(c0, m.ptxtSpace);
+    m.intFactor = (long)(((unsigned __int128)(unsigned long)m.intFactor * (unsigned long)Ctxt::invMod(c0 / d, m.ptxtSpace)) % (unsigned long)m.ptxtSpace);
+    if (d == 1) return;
+    const long cc = Ctxt::balRem(d, m.ptxtSpace);
+    m.noiseBound = m.noiseBound * XD((double)std::labs(cc));
+    for (long r : m.primeSet) scaleRow(a, r, resid(cc, r));
+  }
+  void negate(Term& a) {   // Ctxt::negate
+    for (auto& v : a.s) for (long r : a.meta.primeSet) { const u64 q = (u64)ctx_.ithPrime(r); v[(size_t)r] = (q - v[(size_t)r]) % q; }
+  }
+  void reducePtxtSpace(Term& a, long P) {   // Ctxt::reducePtxtSpace
+    if (!ok) return;
+    if (std::gcd(a.meta.ptxtSpace, P) <= 1) { ok = false; return; }
+    a.meta.reducePtxtSpace(P);
+  }
+  // dst = the combination, in one call: dst's parts are replaced by new ones over the term's primeSet and its metadata
+  // set as Ctxt::operator= sets it from the loop's result (the mod-switch and key-switch statistics only where nonzero)
+  bool form(const Term& a, Ctxt& dst) {
+    if (!ok || &dst.pubKey != &a.meta.pubKey) return false;
+    const std::vector<int32_t> U = a.meta.primeSet.vec();
+    const size_t nU = U.size(), nin = in_.size();
+    std::vector<u64> scal(nin * nU, 0);
+    for (size_t k = 0; k < nin; k++) for (size_t r = 0; r < nU; r++) scal[k * nU + r] = a.s[k][(size_t)U[r]];
+    std::vector<hb_poly*> in0, in1;
+    for (const Ctxt* c : in_) { in0.push_back(c->parts[0].dcrt.handle()); in1.push_back(c->parts[1].dcrt.handle()); }
+    std::vector<CtxtPart> out;
+    out.reserve(3);   // a later product adds a third part: no reallocation, which would copy the two parts through the device
+    out.emplace_back(ctx_, a.meta.primeSet, SKHandle());
+    out.emplace_back(ctx_, a.meta.primeSet, SKHandle(1, 1, keyID_));
+    hb_poly* o0[1] = {out[0].dcrt.handle()}; hb_poly* o1[1] = {out[1].dcrt.handle()};
+    check(hb_ctxt_scaled_sums(in0.data(), in1.data(), (int)nin, o0, o1, 1, 1, U.data(), (int)nU, scal.data(), nullptr, 0));
+    dst.parts.swap(out);
+    const Ctxt& m = a.meta;
+    dst.primeSet = m.primeSet; dst.ptxtSpace = m.ptxtSpace; dst.noiseBound = m.noiseBound;
+    dst.intFactor = m.intFactor; dst.ratFactor = m.ratFactor; dst.ptxtMag = m.ptxtMag;
+    if (m.lastKSNoiseRatio != 0) dst.lastKSNoiseRatio = m.lastKSNoiseRatio;
+    if (m.lastModSwitchRatio != 0) dst.lastModSwitchRatio = m.lastModSwitchRatio;
+    return true;
+  }
+
+ private:
+  std::vector<const Ctxt*> in_;
+  const Context& ctx_;
+  size_t np_;
+  long keyID_ = 0;
+  static Ctxt metaOf(const Ctxt& c) {
+    Ctxt m(c.pubKey, c.ptxtSpace);
+    m.primeSet = c.primeSet; m.noiseBound = c.noiseBound; m.intFactor = c.intFactor; m.ratFactor = c.ratFactor; m.ptxtMag = c.ptxtMag;
+    m.lastKSNoiseRatio = c.lastKSNoiseRatio; m.lastModSwitchRatio = c.lastModSwitchRatio;
+    return m;
+  }
+  u64 resid(long v, long r) const { const long q = ctx_.ithPrime(r); long x = v % q; return (u64)(x < 0 ? x + q : x); }
+  void scaleRow(Term& a, long r, u64 f) {
+    const u64 q = (u64)ctx_.ithPrime(r);
+    for (auto& v : a.s) v[(size_t)r] = (u64)((unsigned __int128)v[(size_t)r] * f % q);
+  }
+  bool modUp(Term& a, const IndexSet& d) {   // Ctxt::modUpToSet's arithmetic
+    if (empty(d)) return true;
+    for (long r : a.meta.primeSet) {
+      u64 f = 1;
+      const u64 q = (u64)ctx_.ithPrime(r);
+      for (long j : d) f = (u64)((unsigned __int128)f * ((u64)ctx_.ithPrime(j) % q) % q);
+      scaleRow(a, r, f);
+    }
+    const double f = a.meta.pubKey.logOfProduct(d);
+    a.meta.noiseBound = a.meta.noiseBound * XD::exp(f);
+    a.meta.ratFactor = a.meta.ratFactor * XD::exp(f);
+    a.meta.primeSet.insert(d);
+    if (!a.meta.verifyPrimeSet()) ok = false;
+    return ok;
+  }
+  void mulInt(Term& a, long e) {   // Ctxt::mulIntFactor's arithmetic
+    if (e == 1) return;
+    Ctxt& m = a.meta;
+    m.intFactor = (long)(((unsigned __int128)(unsigned long)m.intFactor * (unsigned long)e) % (unsigned long)m.ptxtSpace);
+    const long b = Ctxt::balRem(e, m.ptxtSpace);
+    for (long r : m.primeSet) scaleRow(a, r, resid(b, r));
+    m.noiseBound = m.noiseBound * XD((double)std::labs(b));
+  }
+};
+
+namespace detail {
+// the powerings of extractDigits: x^p in spirit (src/extractDigits.cpp:91-97)
+inline void powerDigit(Ctxt& d, const std::vector<long>& x2p) {
+  HB_NTIMER_START(digit_power, d.context.handle());
+  const long p = d.context.getP();
+  if (p == 2) d.square();
+  else if (p == 3) d.cube();
+  else polyEval(d, x2p, d);
+}
+// tmp = c - sum_j in[j] with a divideByP after each step (src/extractDigits.cpp:90-109), as transcribed
+inline void digitChainLoop(Ctxt& dst, const Ctxt& c, const std::vector<const Ctxt*>& sub) {
+  Ctxt tmp(c.pubKey, c.ptxtSpace);
+  tmp = c;
+  for (const Ctxt* d : sub) { tmp -= *d; tmp.divideByP(); }
+  dst = tmp;
+}
+// the same chain in one hb_ctxt_scaled_sums call; false, with nothing launched, where one call cannot reproduce it
+inline bool digitChainFused(Ctxt& dst, const Ctxt& c, const std::vector<const Ctxt*>& sub) {
+  std::vector<const Ctxt*> in{&c};
+  in.insert(in.end(), sub.begin(), sub.end());
+  LinearChain L(in);
+  if (!L.ok) return false;
+  LinearChain::Term t = L.term(0);
+  for (size_t j = 0; j < sub.size(); j++) { L.add(t, L.term(j + 1), true); L.divideByP(t); }
+  return L.form(t, dst);
+}
+// Chen and Han's digit: G(tmp) (src/extractDigits.cpp:283)
+inline void liftDigit(Ctxt& d, const std::vector<long>& G, const Ctxt& tmp) {
+  HB_NTIMER_START(digit_lift, d.context.handle());
+  polyEval(d, G, tmp);
+}
+inline void digitChain(Ctxt& dst, const Ctxt& c, const std::vector<const Ctxt*>& sub, bool fused) {
+  if (sub.empty()) { dst = c; return; }
+  HB_NTIMER_START(digit_chain, c.context.handle());
+  if (!fused || !digitChainFused(dst, c, sub)) digitChainLoop(dst, c, sub);
+}
+}  // namespace detail
+
+// hb::extractDigits (src/extractDigits.cpp:70-129): digits[j] holds the j-th base-p digit of the slots of c (integers mod
+// p^r), at plaintext space p^(r-j).  Round i powers digits 0..i-1 (square for p = 2, cube for p = 3, the digit polynomial
+// through polyEval otherwise) and forms c minus them, divided by p after each, in one hb_ctxt_scaled_sums call.
+// fused = false runs the chains as transcribed (the reference the tests compare against).
+inline void extractDigits(std::vector<Ctxt>& digits, const Ctxt& c, long r = 0, bool fused = true) {
+  const long rr = c.effectiveR();
+  if (r <= 0 || r > rr) r = rr;
+  const long p = c.context.getP();
+  std::vector<long> x2p;
+  if (p > 3) x2p = xd::buildDigitPolynomial(p, r);
+  Ctxt tmp(c.pubKey, c.ptxtSpace);
+  digits.resize((size_t)r, tmp);
+  for (long i = 0; i < r; i++) {
+    std::vector<const Ctxt*> sub;
+    for (long j = 0; j < i; j++) { detail::powerDigit(digits[(size_t)j], x2p); sub.push_back(&digits[(size_t)j]); }
+    detail::digitChain(digits[(size_t)i], c, sub, fused);
+  }
+}
+
+// hb::extendExtractDigits (src/extractDigits.cpp:225-308), Chen and Han's variant: c holds integers mod p^(r+e) in its
+// slots; digits[i] = G_{e+r-i}(the i-th chain), at plaintext space p^(e+r-i).  Each chain subtracts whichever of digits[j]
+// and the powered digits0[j] has more capacity, as HElib does, in one hb_ctxt_scaled_sums call.
+inline void extendExtractDigits(std::vector<Ctxt>& digits, const Ctxt& c, long r, long e, bool fused = true) {
+  const long p = c.context.getP();
+  std::vector<long> x2p;
+  if (p > 3) x2p = xd::buildDigitPolynomial(p, r);
+  std::vector<std::vector<long>> G((size_t)std::max(0L, r));
+  for (long i = 0; i < r; i++) G[(size_t)i] = xd::chenHanMagicPoly(p, e + r - i);
+  Ctxt tmp(c.pubKey, c.ptxtSpace);
+  digits.resize((size_t)r, tmp);
+  std::vector<Ctxt> digits0((size_t)r, tmp);
+  for (long i = 0; i < r; i++) {
+    std::vector<const Ctxt*> sub;
+    for (long j = 0; j < i; j++) {
+      if (digits[(size_t)j].capacity() >= digits0[(size_t)j].capacity()) sub.push_back(&digits[(size_t)j]);
+      else { detail::powerDigit(digits0[(size_t)j], x2p); sub.push_back(&digits0[(size_t)j]); }
+    }
+    detail::digitChain(digits0[(size_t)i], c, sub, fused);
+    detail::liftDigit(digits[(size_t)i], G[(size_t)i], digits0[(size_t)i]);
+  }
+}
+
+namespace detail {
+// extractDigitsThin's final combination (src/recryption.cpp:852-867 and 881-907): from `top` (the Chen-Han branch's
+// chain, or the highest selected digit) down, then the p = 2 bit, the negation and the bottom digits, mod p^r
+struct ThinPlan {
+  long start = -1;   // -1: top = unpacked - scratch[0..botHigh) with a divideByP after each (Chen-Han); else scratch[start]
+  long lo = 0;       // the basic branch's digits start-1 .. lo, each after a multByP
+  long botHigh = 0, r = 0, ePrime = 0, p = 0;
+};
+inline void thinCombineLoop(Ctxt& unpacked, const std::vector<Ctxt>& s, const ThinPlan& P) {
+  if (P.start < 0) {
+    for (long j = 0; j < P.botHigh; j++) { unpacked -= s[(size_t)j]; unpacked.divideByP(); }
+  } else {
+    unpacked = s[(size_t)P.start];
+    for (long j = P.start - 1; j >= P.lo; --j) { unpacked.multByP(); unpacked += s[(size_t)j]; }
+  }
+  if (P.p == 2 && P.botHigh > 0) unpacked += s[(size_t)P.botHigh - 1];
+  unpacked.negate();
+  if (P.r > P.ePrime) {
+    const long topLow = P.r - 1 - P.ePrime;
+    Ctxt tmp = s.at((size_t)topLow);
+    for (long j = topLow - 1; j >= 0; --j) { tmp.multByP(); tmp += s[(size_t)j]; }
+    if (P.ePrime > 0) tmp.multByP(P.ePrime);
+    unpacked += tmp;
+  }
+  unpacked.reducePtxtSpace(xd::power(P.p, P.r));
+}
+inline bool thinCombineFused(Ctxt& unpacked, const std::vector<Ctxt>& s, const ThinPlan& P) {
+  std::vector<const Ctxt*> in;
+  if (P.start < 0) in.push_back(&unpacked);
+  for (const Ctxt& x : s) in.push_back(&x);
+  LinearChain L(in);
+  if (!L.ok) return false;
+  const size_t o = P.start < 0 ? 1 : 0;   // input index of scratch[0]
+  auto S = [&](long j) { return L.term(o + (size_t)j); };
+  LinearChain::Term t = P.start < 0 ? L.term(0) : S(P.start);
+  if (P.start < 0) for (long j = 0; j < P.botHigh; j++) { L.add(t, S(j), true); L.divideByP(t); }
+  else for (long j = P.start - 1; j >= P.lo; --j) { L.multByP(t); L.add(t, S(j)); }
+  if (P.p == 2 && P.botHigh > 0) L.add(t, S(P.botHigh - 1));
+  L.negate(t);
+  if (P.r > P.ePrime) {
+    const long topLow = P.r - 1 - P.ePrime;
+    LinearChain::Term b = S(topLow);
+    for (long j = topLow - 1; j >= 0; --j) { L.multByP(b); L.add(b, S(j)); }
+    if (P.ePrime > 0) L.multByP(b, P.ePrime);
+    L.add(t, b);
+  }
+  L.reducePtxtSpace(t, xd::power(P.p, P.r));
+  return L.form(t, unpacked);
+}
+}  // namespace detail
+
+// hb::extractDigitsThin (src/recryption.cpp:793-909): ctxt's slots hold integers mod p^(botHigh+r); ctxt becomes
+// -(digits botHigh .. botHigh+r-1, as one integer mod p^r) plus, for r > ePrime, the digits below r-ePrime times p^ePrime,
+// at plaintext space p^r.  The cost rule picks Chen and Han's method or the basic one; chenHan > 0 forces the former and
+// chenHan < 0 the latter (HElib's global fhe_force_chen_han).  The final combination is one hb_ctxt_scaled_sums call.
+inline void extractDigitsThin(Ctxt& ctxt, long botHigh, long r, long ePrime, long chenHan = 0, bool fused = true) {
+  Ctxt unpacked(ctxt);
+  unpacked.cleanUp();
+  std::vector<Ctxt> scratch;
+  const long p = ctxt.context.getP();
+  long topHigh = botHigh + r - 1;
+  bool useChenHan = false;
+  if (r > 1) {   // degree of Chen-Han p^(bot-1)(p-1)r; of the basic method p^(bot-1)p^r, or p^(bot-1)p^(r-1) for a free bit
+    const double chenHanCost = std::log((double)(p - 1)) + std::log((double)r);
+    const double basicCost = (p == 2 && r > 2 && botHigh + r > 2) ? (r - 1) * std::log((double)p) : r * std::log((double)p);
+    const double thresh = p == 2 ? 1.75 : 1.5;   // squaring is cheaper: p = 2 leans to the basic method
+    if (basicCost > thresh * chenHanCost) useChenHan = true;
+  }
+  if (chenHan > 0) useChenHan = true;
+  else if (chenHan < 0) useChenHan = false;
+  detail::ThinPlan plan;
+  plan.botHigh = botHigh; plan.r = r; plan.ePrime = ePrime; plan.p = p;
+  if (useChenHan) {
+    extendExtractDigits(scratch, unpacked, botHigh, r, fused);
+  } else {
+    if (p == 2 && r > 2 && topHigh + 1 > 2) topHigh--;   // for p = 2 the top bit comes for free
+    extractDigits(scratch, unpacked, topHigh + 1, fused);
+    if (topHigh >= (long)scratch.size()) topHigh = (long)scratch.size() - 1;   // not enough digits: HElib warns and goes on
+    plan.start = topHigh;
+    plan.lo = botHigh;
+  }
+  {
+    HB_NTIMER_START(thin_combine, ctxt.context.handle());
+    if (!fused || !detail::thinCombineFused(unpacked, scratch, plan)) detail::thinCombineLoop(unpacked, scratch, plan);
+  }
+  ctxt = unpacked;
 }
 
 }  // namespace hb
